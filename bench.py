@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 pairwise string-similarity hot path.
+"""bench.py -- headline benchmark of the H100 pairwise string-similarity hot path.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): char-trigram TF-IDF top-10, company-names self-match,
 n = 100 000 -- on the reference's own data/company_names.json (shipped as a test fixture under
@@ -18,6 +18,11 @@ N > 1 (torchrun, one rank per GPU, NCCL): weak scaling.  The to_list grows to N 
 row-sharded (rank r owns block r); the from_list stays the first block (100 000 names), scored
 against all shards with the global diagonal excluded -- i.e. one from-row-block of the N*100k
 self-match.  Per-GPU work is fixed; one all-reduce (df) + one all-gather (top-k) per step.
+
+Every timed loop (the headline steps, the e2e leg and each sub-record) runs --warmup untimed and --steps timed
+iterations.  --dump-outputs DIR writes, after the timed steps, what the last headline step computed -- the top-k
+indices and scores a caller of that path receives -- as DIR/top_idx.npy and DIR/top_val.npy (float64, n x 10); the
+inputs are the fixture or seeded, so two builds can be compared output for output.
 
 Prints ONE JSON line on rank 0 (see the repository README / DESIGN.md for the keys).
 """
@@ -53,6 +58,7 @@ def parse():
     ap.add_argument("--skip", default="", help="comma list of sub-records to skip: c3,c4,c5,e2e")
     ap.add_argument("--c5-n", type=int, default=1_000_000, help="rows per list of the c5 sub-record")
     ap.add_argument("--synthetic", action="store_true", help="force the synthetic stand-in data")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's top-k as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -132,7 +138,7 @@ def run_reference(args):
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clocks / throttle reasons DURING the timed region (B200_PROFILING.md).  Sampled in-process through NVML
+    """SM clocks / throttle reasons DURING the timed region.  Sampled in-process through NVML
     (nvidia_ml_py) every 50 ms: an external `nvidia-smi -lms` loop takes the driver lock for milliseconds per query and
     showed up as +4 ms outliers in 14 ms steps.  Falls back to nvidia-smi if NVML is unavailable."""
     REASONS = {"hw_slowdown": 0x8, "sw_power_cap": 0x4, "sw_thermal_slowdown": 0x20, "hw_thermal_slowdown": 0x40}
@@ -227,7 +233,7 @@ def hbm_peak():
     if os.path.exists(peaks_path):
         pk = json.load(open(peaks_path))
         return pk, float(pk["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return {}, 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return {}, 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 def timed(fn, warmup, steps, sync, flush=None):
@@ -274,7 +280,7 @@ def load_names(args, rank, world):
 
 
 # ---- sub-records -------------------------------------------------------------------------------------
-def sub_c3(dev, local_rank, sync, flush):
+def sub_c3(args, dev, local_rank, sync, flush):
     """BASELINE configs[2]: all-pairs edit distance on movie_titles (Netflix 6 172 x IMDB 80 852), per-row best match.
     Device-timed from staged blobs (EditQueries / EditTargets) to the arg-best arrays; integer-ALU roofline against the
     INT32 issue rate measured by pfz_int_alu_probe in this run."""
@@ -291,7 +297,7 @@ def sub_c3(dev, local_rank, sync, flush):
     w32 = np.where(Q.lens <= 32, 1, 2 * np.ceil(Q.lens / 64.0)).astype(np.float64)
     word_steps32 = float(w32.sum()) * float(tl.sum())
     # probe: INT32 lane-ops/s of the ALU pipe (LOP3 + IADD chains)
-    scratch = torch.empty(148 * 8 * 256 * 2, dtype=torch.int32, device=dev)
+    scratch = torch.empty(torch.cuda.get_device_properties(dev).multi_processor_count * 8 * 256, dtype=torch.int32, device=dev)
     nops = ctypes.c_int64(0)
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     probe_ms = timed(lambda: _lib.call("pfz_int_alu_probe", 4096, ctypes.c_void_p(scratch.data_ptr()), ctypes.byref(nops), st), 2, 5, sync)
@@ -305,7 +311,7 @@ def sub_c3(dev, local_rank, sync, flush):
         res = {}
         def run():
             res["r"] = editdist.edit_argbest_staged(Q, T, metric)
-        ms = timed(run, 2, 5, sync, flush)
+        ms = timed(run, args.warmup, args.steps, sync, flush)
         t = float(np.median(ms)) * 1e-3
         alg_ops = word_steps32 * ops
         out[key] = {"ms": t * 1e3, "ms_each": [round(x, 3) for x in ms], "pairs_per_s": pairs / t, "gcups": cells / t / 1e9,
@@ -319,7 +325,7 @@ def sub_c3(dev, local_rank, sync, flush):
     return out
 
 
-def sub_c4(dev, local_rank, sync, flush, peaks):
+def sub_c4(args, dev, local_rank, sync, flush, peaks):
     """BASELINE configs[3]: dense cosine top-10, 100k x 100k x 768 random unit vectors (bf16 in, fp32 accumulate)."""
     import torch
     from polyfuzz_b200 import dense
@@ -329,18 +335,19 @@ def sub_c4(dev, local_rank, sync, flush, peaks):
     x, _ = dense.to_bf16_rows(X, True); y, _ = dense.to_bf16_rows(Y, True)
     del X, Y
     sampler = ClockSampler(local_rank)
-    ms = timed(lambda: dense.dense_topk(x, y, k, 0.0), 3, 10, sync, flush)
+    ms = timed(lambda: dense.dense_topk(x, y, k, 0.0), args.warmup, args.steps, sync, flush)
     clocks = sampler.stop()
     t = float(np.median(ms)) * 1e-3
     flops = 2.0 * n * n * d
-    burst = float(peaks.get("bf16_tflops", 1590.0)); sust = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    burst = float(peaks.get("bf16_tflops", 989.0)); sust = float(peaks.get("bf16_tflops_sustained", 989.0))
     ach = flops / t / 1e12
-    return {"workload": "dense cosine top-10, 100k x 100k x 768 random unit vectors, bf16 tcgen05 (BASELINE configs[3])", "data": "synthetic",
+    return {"workload": "dense cosine top-10, 100k x 100k x 768 random unit vectors, bf16 wgmma (BASELINE configs[3])", "data": "synthetic",
             "n_from": n, "n_to": n, "d": d, "top_n": k, "ms": t * 1e3, "ms_each": [round(v, 3) for v in ms],
             "value": float(n) * n / t, "unit": UNIT, "tflops": ach,
             "roofline": {"bound": "tensor", "achieved": ach, "peak": burst, "unit": "TFLOP/s", "frac": ach / burst,
                          "peak_sustained": sust, "frac_of_sustained": ach / sust,
-                         "peak_source": "MEASURED_PEAKS.json bf16_tflops (cuBLAS burst) / bf16_tflops_sustained" if peaks else "fallback"},
+                         "peak_source": "MEASURED_PEAKS.json bf16_tflops (cuBLAS burst) / bf16_tflops_sustained" if peaks
+                         else "H100 SXM data sheet, dense bf16 at 700 W"},
             "clocks": clocks}
 
 
@@ -367,13 +374,13 @@ def sub_c5(args, dev, rank, local_rank, world, comm, barrier, flush, peak):
                                                      comm=comm, timings=k2_events if rec else None, n_docs_total=2 * n)
         res.update(idx=idx, val=val, vec=vec, csr=csr_to, index=index)
     sampler = ClockSampler(local_rank, recording=False) if rank == 0 else None
-    for _ in range(2):
+    for _ in range(args.warmup):
         flush.zero_(); step(False)
     barrier()
     if sampler:
         sampler.recording = True
     ms = []
-    for _ in range(3):
+    for _ in range(args.steps):
         flush.zero_(); barrier()
         e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
         e0.record(); step(True); e1.record()
@@ -478,6 +485,10 @@ def run_b200(args):
         barrier()
         step_ms.append(e0.elapsed_time(e1))
     launches = _lib.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "top_idx.npy"), result["idx"].cpu().numpy().astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "top_val.npy"), result["val"].cpu().numpy().astype(np.float64))
     total_ms = torch.tensor([float(np.sum(step_ms))], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(total_ms, op=dist.ReduceOp.MAX)
@@ -498,14 +509,13 @@ def run_b200(args):
         return m.match(from_list)
 
     e2e_ms = []
-    e2e_steps = max(3, args.steps)
-    for it in range(2 + e2e_steps):
+    for it in range(args.warmup + args.steps):
         flush.zero_()
         barrier()
         e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
         e0.record(); df = e2e_step(); e1.record()
         barrier()
-        if it >= 2:
+        if it >= args.warmup:
             e2e_ms.append(e0.elapsed_time(e1))
     e2e_total = torch.tensor([float(np.sum(e2e_ms))], dtype=torch.float64, device=dev)
     if world > 1:
@@ -518,9 +528,9 @@ def run_b200(args):
     # ---- sub-records (other BASELINE configs), every one with its own clock record ----------------
     subs = {}
     if world == 1 and "c3" not in skip:
-        subs["c3"] = sub_c3(dev, local_rank, torch.cuda.synchronize, flush)
+        subs["c3"] = sub_c3(args, dev, local_rank, torch.cuda.synchronize, flush)
     if world == 1 and "c4" not in skip:
-        subs["c4"] = sub_c4(dev, local_rank, torch.cuda.synchronize, flush, peaks)
+        subs["c4"] = sub_c4(args, dev, local_rank, torch.cuda.synchronize, flush, peaks)
     if "c5" not in skip:
         keep_main = dict(result)
         subs["c5"] = sub_c5(args, dev, rank, local_rank, world, comm, barrier, flush, peak)
@@ -553,16 +563,9 @@ def run_b200(args):
     b_alg = P * (4 + s_bytes) + nnz_from * (4 + s_bytes) + n * TOP_N * 12
     b_alg_fp64 = P * 12 + nnz_from * 12 + n * TOP_N * 12
     k2_avg_ms = float(np.mean(k2_ms))
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "k2_ncu_summary.json")
-    if os.path.exists(tpath):
-        try:
-            traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
-        except Exception:
-            traffic = None
     achieved = b_alg / (k2_avg_ms * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": "K2 pfz_spcos_topk (variant %s)" % variant, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "weight_bytes_per_posting": s_bytes,
                 "algorithmic_bytes_per_launch": b_alg, "postings_per_launch": P, "kernel_ms_avg": k2_avg_ms,
                 "kernel_share_of_step": k2_avg_ms / ms_per_step,

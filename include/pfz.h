@@ -1,4 +1,4 @@
-/* pfz.h -- C ABI of libpfz.so: the B200 (sm_100a) pairwise string-similarity hot path that
+/* pfz.h -- C ABI of libpfz.so: the H100 (sm_90a) pairwise string-similarity hot path that
  * drops in behind PolyFuzz's BaseMatcher plugins.
  *
  * The reference (MaartenGr/PolyFuzz @ v0.4.3) is pure Python and has no FFI of its own; its hot
@@ -15,7 +15,7 @@
  *   - the last argument is the CUDA stream (cudaStream_t passed as void*); all work is enqueued on
  *     it and nothing synchronises unless stated;
  *   - strings travel as UTF-32 code points: `blob` (uint32) + `offsets` (int64, n+1 entries);
- *   - there is NO CPU fallback: on a machine without an sm_100 device the calls fail.
+ *   - there is NO CPU fallback: on a machine without an sm_90 device the calls fail.
  */
 #ifndef PFZ_H
 #define PFZ_H
@@ -255,7 +255,7 @@ int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, in
                      int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
- * K4  dense cosine top-k for pre-computed embeddings (bf16 tcgen05 GEMM fed by TMA, top-k fused into the
+ * K4  dense cosine top-k for pre-computed embeddings (bf16 wgmma GEMM fed by TMA, top-k fused into the
  * epilogue).  Replaces the dense branch polyfuzz/models/_utils.py:94-102 (sklearn cosine_similarity +
  * argsort) reached from polyfuzz/models/_embeddings.py:127-131.
  * ---------------------------------------------------------------------------------------------- */

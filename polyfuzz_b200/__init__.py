@@ -1,4 +1,4 @@
-"""polyfuzz_b200 -- B200-native (sm_100a) pairwise string-similarity hot path behind PolyFuzz's
+"""polyfuzz_b200 -- H100-native (sm_90a) pairwise string-similarity hot path behind PolyFuzz's
 BaseMatcher plugin API.  See DESIGN.md / INTEGRATION.md."""
 from .matchers import BaseMatcher, TFIDF, RapidFuzz, EditDistance, Embeddings  # noqa: F401
 
@@ -7,7 +7,7 @@ __version__ = "0.1.0"
 
 def install():
     """Make the reference's string shortcuts -- PolyFuzz("TF-IDF"), PolyFuzz("EditDistance"), PolyFuzz("Embeddings")
-    (polyfuzz/polyfuzz.py:124-133) -- construct the B200 matchers: the names the unmodified orchestrator looks up in its own
+    (polyfuzz/polyfuzz.py:124-133) -- construct this package's matchers: the names the unmodified orchestrator looks up in its own
     module (and polyfuzz.models) are rebound to the classes of this package.  No reference source is modified."""
     import polyfuzz.models as pm
     import polyfuzz.polyfuzz as pp

@@ -70,7 +70,7 @@ int pfz_frame_tail_count(const int32_t *top_idx, const double *top_val, int32_t 
     cudaStream_t st = as_stream(stream);
     const int words_per_col = (n + 31) / 32;
     const int64_t total = (int64_t)k * words_per_col * 32;
-    int grid = (int)((total + 255) / 256); if (grid > 148 * 16) grid = 148 * 16;
+    int grid = (int)((total + 255) / 256); if (grid > SM_COUNT * 16) grid = SM_COUNT * 16;
     PFZ_CUDA_OK(cudaMemsetAsync(lens_pos + (int64_t)n * k, 0, sizeof(int32_t), st));
     tail_count_kernel<<<grid, 256, 0, st>>>(top_idx, top_val, n, k, to_offsets, sims, lens_pos, bitmap, words_per_col);
     PFZ_LAUNCH_OK();
@@ -81,7 +81,7 @@ int pfz_frame_tail_copy(const int32_t *top_idx, int32_t n, int32_t k, const int3
                         int64_t *offsets, uint8_t *data, void *stream) {
     if (n <= 0 || k <= 0) return 0;
     const int64_t n_ent = (int64_t)n * k;
-    int grid = (int)((n_ent * 32 + 255) / 256); if (grid > 148 * 16) grid = 148 * 16;
+    int grid = (int)((n_ent * 32 + 255) / 256); if (grid > SM_COUNT * 16) grid = SM_COUNT * 16;
     tail_copy_kernel<<<grid, 256, 0, as_stream(stream)>>>(top_idx, n, k, to_blob, to_offsets, pos, offsets, data);
     PFZ_LAUNCH_OK();
     return 0;

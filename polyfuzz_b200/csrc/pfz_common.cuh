@@ -1,4 +1,4 @@
-// pfz_common.cuh -- shared helpers for libpfz.so (sm_100a only).
+// pfz_common.cuh -- shared helpers for libpfz.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,6 +31,9 @@ extern unsigned long long g_launches;   // kernels launched by this library (ben
 static inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s); }
 
 constexpr unsigned FULL = 0xffffffffu;
+
+// SMs of an H100 SXM: caps the grids of grid-stride kernels (a few resident blocks per SM)
+constexpr int SM_COUNT = 132;
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 

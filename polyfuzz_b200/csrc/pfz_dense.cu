@@ -1,15 +1,21 @@
-// pfz_dense.cu -- K4: dense cosine top-k for pre-computed embeddings: C = X * Y^T on the 5th-generation
-// tensor cores (tcgen05.mma, bf16 in, fp32 accumulate in TMEM) fed by TMA, with the per-row top-k fused
-// into the epilogue so the n_from x n_to score matrix never exists in memory.
+// pfz_dense.cu -- K4: dense cosine top-k for pre-computed embeddings: C = X * Y^T on the Hopper tensor cores
+// (wgmma, bf16 in, fp32 accumulate in registers) fed by TMA, with the per-row top-k fused into the epilogue so
+// the n_from x n_to score matrix never exists in memory.
 //
 // Replaces the dense branch of polyfuzz/models/_utils.py:94-102 (sklearn cosine_similarity + argsort) as
 // reached from polyfuzz/models/_embeddings.py:127-131 when the caller supplies embeddings.
 //
-// CTA = 128 from-rows (one TMEM lane per row).  Per 256-wide to-tile: K loop of 64-element (128-byte,
-// SWIZZLE_128B) TMA boxes through a 4-stage shared-memory ring, tcgen05.mma M=128,N=256,K=16 issued by one
-// thread, accumulator double-buffered in TMEM (2 x 256 columns) so the epilogue of tile t overlaps the MMAs of
-// tile t+1.  Warp roles: 0 = TMA producer, 1 = MMA issuer, 2 = TMEM allocator, 4..7 = epilogue (thread =
-// row, sorted top-k in registers, key (score desc, index asc)).
+// CTA = 128 from-rows.  Per DN-wide to-tile: K loop of 64-element (128-byte, SWIZZLE_128B) TMA boxes through a
+// shared-memory ring of full / empty mbarriers.  Warps 0-7 are two consumer warpgroups (from-rows 0-63 and 64-127
+// of the block), each issuing wgmma m64nDNk16 into DN/2 fp32 registers per thread; warp 8 is the TMA producer.
+// The wgmma accumulator layout gives each thread two rows (r and r + 8 of its warp's 16) and DN/4 columns of each:
+// the thread keeps a sorted top-k per row over its columns (key: score desc, index asc), and the four threads of a
+// quad merge their lists with shuffles when a (row block, split) unit is done.  DN = 128 keeps the 64 accumulators and
+// both top-k lists in registers: 9 warps per CTA leave 168 registers a thread, and DN = 256 spilled.
+//
+// Cluster variant (MCAST): a pair of CTAs (cluster of 2) works on two adjacent 128-row blocks against the same
+// to-tiles.  Each CTA loads one half of the Y tile and multicasts it into both CTAs' shared memory, which halves
+// the to-operand L2 -> SM traffic per CTA; a stage is refilled only once the consumers of both CTAs released it.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -17,9 +23,11 @@
 
 namespace pfz {
 
-constexpr int DM = 128, DN = 256, DK = 64, DSTAGES = 4, UMMA_K = 16;
-constexpr int A_BYTES = DM * DK * 2, B_BYTES = DN * DK * 2;          // 16 KB, 32 KB
-constexpr int DENSE_THREADS = 256;
+constexpr int DM = 128, DN = 128, DK = 64, WG_K = 16, DSTAGES = 6;
+constexpr int A_BYTES = DM * DK * 2, B_BYTES = DN * DK * 2;          // 16 KB, 16 KB
+constexpr int DENSE_THREADS = 288;                                     // 2 consumer warpgroups + 1 producer warp
+constexpr int DENSE_CONSUMER_WARPS = 8;
+constexpr size_t DENSE_SMEM = (size_t)DSTAGES * (A_BYTES + B_BYTES) + 2 * DSTAGES * 8 + 1024;
 
 __device__ __forceinline__ unsigned s32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar), "r"(count)); }
@@ -27,6 +35,10 @@ __device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(unsigned bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory"); }
+__device__ __forceinline__ void mbar_arrive_cta(unsigned bar, unsigned cta) {      // the barrier at the same offset in CTA `cta` of the cluster
+    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\tmbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+                 :: "r"(bar), "r"(cta) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
     asm volatile("{\n\t.reg .pred p;\n\tLAB_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE;\n\tbra LAB_WAIT;\n\tDONE:\n\t}"
                  :: "r"(bar), "r"(parity) : "memory");
@@ -35,46 +47,50 @@ __device__ __forceinline__ void tma_load_2d(unsigned dst, const CUtensorMap *map
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  :: "r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(unsigned bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(bar) : "memory");
+// same box into the same shared-memory offset of every CTA in `mask`, completing bytes on each CTA's barrier at `bar`
+__device__ __forceinline__ void tma_load_2d_mcast(unsigned dst, const CUtensorMap *map, int c0, int c1, unsigned bar, unsigned short mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;"
+                 :: "r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar), "h"(mask) : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]^T, kind::f16 (bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void tc_mma(unsigned d_tmem, uint64_t adesc, uint64_t bdesc, unsigned idesc, unsigned accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+__device__ __forceinline__ unsigned cluster_ctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 // shared-memory matrix descriptor: K-major operand, 128-byte swizzle, 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t umma_desc(unsigned smem_addr) {
+__device__ __forceinline__ uint64_t wgmma_desc(unsigned smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);               // start address  (bits 0-13)
     d |= (uint64_t)1 << 16;                                    // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;                          // stride byte offset (bits 32-45)
-    d |= (uint64_t)1 << 46;                                    // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                                    // layout type: SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                                    // layout: SWIZZLE_128B
     return d;
 }
-// instruction descriptor, kind::f16: D=f32, A=B=bf16, both K-major, M=128, N=256
-__device__ __forceinline__ unsigned umma_idesc() {
-    unsigned d = 0;
-    d |= 1u << 4;                       // c_format = F32
-    d |= 1u << 7;                       // a_format = BF16
-    d |= 1u << 10;                      // b_format = BF16
-    d |= (unsigned)(DN >> 3) << 17;     // n_dim
-    d |= (unsigned)(DM >> 4) << 24;     // m_dim
-    return d;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int R> __device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
-__device__ __forceinline__ void tmem_ld32(unsigned taddr, unsigned (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-                   "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                   "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// D (+)= A[smem] * B[smem]^T, bf16 inputs, fp32 accumulate; scale_d == 0 overwrites D
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+                 "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
 
 struct DenseParams {
@@ -83,342 +99,169 @@ struct DenseParams {
     int32_t *top_idx; double *top_val;          // [n_splits][n_from][k]
 };
 
+// sorted insert into one row's top-k list; (kv, ki) tracks the k-th key, ki relative to to_base (-1 while not full)
 template <int KMAX>
+__device__ __forceinline__ void topk_insert(float (&tv)[KMAX], int (&ti)[KMAX], float &kv, int &ki, int k, float cv, int ci, long long to_base) {
+#pragma unroll
+    for (int z = 0; z < KMAX; ++z) {
+        if (z < k) {
+            const bool before = cv > tv[z] || (cv == tv[z] && (ti[z] < 0 || ci < ti[z]));
+            if (before) { const float fv = tv[z]; const int fi = ti[z]; tv[z] = cv; ti[z] = ci; cv = fv; ci = fi; }
+            if (z == k - 1) { kv = tv[z]; ki = ti[z] < 0 ? -1 : ti[z] - (int)to_base; }
+        }
+    }
+}
+
+template <int KMAX, bool MCAST>
 __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const __grid_constant__ CUtensorMap map_x,
                                                                           const __grid_constant__ CUtensorMap map_y, const DenseParams P) {
+    constexpr int S = DSTAGES, G = MCAST ? 2 : 1;
     extern __shared__ __align__(1024) unsigned char dsm_raw[];
-    // 128-byte-swizzled TMA/UMMA tiles need 1024-byte alignment: align by hand (the launch adds 1 KB of slack)
+    // 128-byte-swizzled TMA/wgmma tiles need 1024-byte alignment: align by hand (the launch adds 1 KB of slack).  The
+    // offset is the same in every CTA of the launch, which the multicast relies on.
     unsigned char *dsm = dsm_raw + ((1024u - (s32(dsm_raw) & 1023u)) & 1023u);
-    // [A stages][B stages] then barriers
     unsigned char *sa = dsm;
-    unsigned char *sb = dsm + DSTAGES * A_BYTES;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(dsm + DSTAGES * (A_BYTES + B_BYTES));
-    // bars: full[0..S), empty[S..2S), tmem_full[2S..2S+2), tmem_empty[2S+2..2S+4)
-    unsigned *tmem_slot = reinterpret_cast<unsigned *>(bars + 2 * DSTAGES + 4);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const unsigned bar0 = s32(bars);
+    unsigned char *sb = dsm + S * A_BYTES;
+    const unsigned bar0 = s32(dsm + S * (A_BYTES + B_BYTES));
     auto full_bar = [&](int s) { return bar0 + 8u * s; };
-    auto empty_bar = [&](int s) { return bar0 + 8u * (DSTAGES + s); };
-    auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * DSTAGES + a); };
-    auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * DSTAGES + 2 + a); };
+    auto empty_bar = [&](int s) { return bar0 + 8u * (S + s); };
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const unsigned rank = MCAST ? cluster_ctarank() : 0u;
 
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < DSTAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 128); }
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < S; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), G * DENSE_CONSUMER_WARPS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" :: "r"(s32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
+    if (MCAST) cluster_sync_all();                                       // the peer's barriers exist before anything signals them
 
-    const int n_units = P.n_mblocks * P.n_splits;
+    // unit = (group of G adjacent row blocks, split); CTA `rank` of a cluster takes row block G * group + rank
+    const int n_groups = (P.n_mblocks + G - 1) / G;
+    const int n_units = n_groups * P.n_splits;
     const int tiles_per = (P.n_ntiles + P.n_splits - 1) / P.n_splits;
     const int n_kblk = (P.d + DK - 1) / DK;
+    const int u0 = blockIdx.x / G, ustep = gridDim.x / G;
 
-    if (warp == 0) {
+    if (warp == DENSE_CONSUMER_WARPS) {
         if (lane == 0) {
             int stage = 0; unsigned phase = 0;
-            for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-                const int mb = u % P.n_mblocks, sp = u / P.n_mblocks;
+            for (int u = u0; u < n_units; u += ustep) {
+                const int mb = (u % n_groups) * G + (int)rank, sp = u / n_groups;
                 const int t_lo = sp * tiles_per, t_hi = min(P.n_ntiles, t_lo + tiles_per);
                 for (int t = t_lo; t < t_hi; ++t) {
                     for (int kb = 0; kb < n_kblk; ++kb) {
                         mbar_wait(empty_bar(stage), phase ^ 1);
                         mbar_expect_tx(full_bar(stage), A_BYTES + B_BYTES);
                         tma_load_2d(s32(sa + stage * A_BYTES), &map_x, kb * DK, mb * DM, full_bar(stage));
-                        tma_load_2d(s32(sb + stage * B_BYTES), &map_y, kb * DK, t * DN, full_bar(stage));
-                        if (++stage == DSTAGES) { stage = 0; phase ^= 1; }
+                        if (MCAST)
+                            tma_load_2d_mcast(s32(sb + stage * B_BYTES) + rank * (B_BYTES / 2), &map_y, kb * DK, t * DN + (int)rank * (DN / 2),
+                                              full_bar(stage), (unsigned short)0x3);
+                        else
+                            tma_load_2d(s32(sb + stage * B_BYTES), &map_y, kb * DK, t * DN, full_bar(stage));
+                        if (++stage == S) { stage = 0; phase ^= 1; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const unsigned idesc = umma_idesc();
-            int stage = 0; unsigned phase = 0; int acc = 0; unsigned acc_phase = 0;
-            for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-                const int sp = u / P.n_mblocks;
-                const int t_lo = sp * tiles_per, t_hi = min(P.n_ntiles, t_lo + tiles_per);
-                for (int t = t_lo; t < t_hi; ++t) {
-                    mbar_wait(tempty_bar(acc), acc_phase ^ 1);            // epilogue drained this accumulator
-                    tc_fence_after();
-                    const unsigned d_tmem = tmem_base + (unsigned)(acc * DN);
-                    for (int kb = 0; kb < n_kblk; ++kb) {
-                        mbar_wait(full_bar(stage), phase);
-                        tc_fence_after();
-                        const uint64_t adesc = umma_desc(s32(sa + stage * A_BYTES));
-                        const uint64_t bdesc = umma_desc(s32(sb + stage * B_BYTES));
-#pragma unroll
-                        for (int kk = 0; kk < DK / UMMA_K; ++kk) {
-                            // advance 16 elements = 32 bytes along K inside the 128-byte swizzled row: +2 in the address field
-                            tc_mma(d_tmem, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), idesc, (kb | kk) ? 1u : 0u);
-                        }
-                        tc_commit(empty_bar(stage));                      // smem slot free once these MMAs retire
-                        if (++stage == DSTAGES) { stage = 0; phase ^= 1; }
-                    }
-                    tc_commit(tfull_bar(acc));                            // accumulator complete
-                    if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-                }
+        __syncwarp();
+    } else {
+        const int wg = warp >> 2;                                        // consumer warpgroup: rows 64 wg .. 64 wg + 63 of the block
+        const int q4 = lane & 3;
+        auto release = [&](int s) {
+            if (lane == 0) {
+                if (MCAST) { mbar_arrive_cta(empty_bar(s), 0); mbar_arrive_cta(empty_bar(s), 1); }
+                else mbar_arrive(empty_bar(s));
             }
-        }
-    } else if (warp >= 4) {
-        const int ew = warp - 4;                                          // == warp % 4: TMEM lane quarter of this warp
-        const int row_in_blk = ew * 32 + lane;
-        int acc = 0; unsigned acc_phase = 0;
-        for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-            const int mb = u % P.n_mblocks, sp = u / P.n_mblocks;
+        };
+        int stage = 0; unsigned phase = 0;
+        for (int u = u0; u < n_units; u += ustep) {
+            const int mb = (u % n_groups) * G + (int)rank, sp = u / n_groups;
             const int t_lo = sp * tiles_per, t_hi = min(P.n_ntiles, t_lo + tiles_per);
-            const int row = mb * DM + row_in_blk;
-            const long long self_col = P.from_base + row - P.to_base;    // local to-column of the diagonal
-            float tv[KMAX]; int ti[KMAX];
+            const int row0 = mb * DM + wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+            float tv[2][KMAX]; int ti[2][KMAX]; float kv[2]; int ki[2];
 #pragma unroll
-            for (int q = 0; q < KMAX; ++q) { tv[q] = P.min_sim; ti[q] = -1; }
-            float kv = P.min_sim; int ki = -1;
+            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                for (int q = 0; q < KMAX; ++q) { tv[h][q] = P.min_sim; ti[h][q] = -1; }
+                kv[h] = P.min_sim; ki[h] = -1;
+            }
             for (int t = t_lo; t < t_hi; ++t) {
-                mbar_wait(tfull_bar(acc), acc_phase);
-                tc_fence_after();
-                const unsigned taddr = tmem_base + ((unsigned)(ew * 32) << 16) + (unsigned)(acc * DN);
-                for (int c0 = 0; c0 < DN; c0 += 32) {
-                    unsigned r[32];
-                    tmem_ld32(taddr + (unsigned)c0, r);
-                    // pass 1 (branch-free, 2-3 instructions per value): which of the 32 scores rank before the k-th key?
-                    // (score desc, index asc); the sentinel (min_sim, -1) makes the test strict while the list is not full
-                    const int colb = t * DN + c0;
-                    unsigned mask = 0u;
+                float acc[DN / 2];
+                int prev = -1;
+                for (int kb = 0; kb < n_kblk; ++kb) {
+                    mbar_wait(full_bar(stage), phase);
+                    const uint64_t ad = wgmma_desc(s32(sa + stage * A_BYTES + wg * (64 * DK * 2)));
+                    const uint64_t bd = wgmma_desc(s32(sb + stage * B_BYTES));
+                    wgmma_fence();
 #pragma unroll
-                    for (int q = 0; q < 32; ++q) {
-                        const float sc = __uint_as_float(r[q]);
-                        if (sc > kv || (sc == kv && colb + q < ki)) mask |= 1u << q;
-                    }
-                    // pass 2 (rare after the first tiles; the insertion code exists once, not 32 times -- the unrolled
-                    // version overflowed the instruction cache and ran ~30x slower)
-                    while (mask) {
-                        const int q = __ffs(mask) - 1; mask &= mask - 1;
-                        float sc = 0.f;
+                    for (int kk = 0; kk < DK / WG_K; ++kk)
+                        // advance 16 elements = 32 bytes along K inside the 128-byte swizzled row: +2 in the address field
+                        wgmma_m64n128(acc, ad + (uint64_t)(kk * 2), bd + (uint64_t)(kk * 2), (kb | kk) ? 1 : 0);
+                    wgmma_commit();
+                    wgmma_wait<1>();                                     // the previous stage's MMAs have retired
+                    if (prev >= 0) release(prev);
+                    prev = stage;
+                    if (++stage == S) { stage = 0; phase ^= 1; }
+                }
+                wgmma_wait<0>();
+                acc_fence(acc);
+                release(prev);
+                // accumulator layout: acc[4 j + 2 h + e] = (row0 + 8 h, column 8 j + 2 q4 + e of the tile)
+                const int colb = t * DN + 2 * q4;
 #pragma unroll
-                        for (int z = 0; z < 32; ++z) if (z == q) sc = __uint_as_float(r[z]);
-                        const int col = colb + q;
-                        if (!(sc > kv || (sc == kv && col < ki))) continue;          // the key may have risen meanwhile
-                        if (col >= P.n_to || (P.self_match && (long long)col == self_col)) continue;
-                        float cv = sc; int ci = (int)(P.to_base + col);
+                for (int h = 0; h < 2; ++h) {
+                    const long long self_col = P.from_base + row0 + 8 * h - P.to_base;   // local to-column of the diagonal
 #pragma unroll
-                        for (int z = 0; z < KMAX; ++z) {
-                            if (z < P.k) {
-                                const bool before = cv > tv[z] || (cv == tv[z] && (ti[z] < 0 || ci < ti[z]));
-                                if (before) { const float fv = tv[z]; const int fi = ti[z]; tv[z] = cv; ti[z] = ci; cv = fv; ci = fi; }
-                                if (z == P.k - 1) { kv = tv[z]; ki = ti[z] < 0 ? -1 : ti[z] - (int)P.to_base; }
-                            }
+                    for (int c = 0; c < DN / 128; ++c) {
+                        // pass 1 (branch-free): which of these 32 scores rank before the k-th key?  (score desc, index asc);
+                        // the sentinel (min_sim, -1) makes the test strict while the list is not full
+                        unsigned mask = 0u;
+#pragma unroll
+                        for (int q = 0; q < 32; ++q) {
+                            const int j = c * 16 + (q >> 1);
+                            const float sc = acc[4 * j + 2 * h + (q & 1)];
+                            if (sc > kv[h] || (sc == kv[h] && colb + 8 * j + (q & 1) < ki[h])) mask |= 1u << q;
+                        }
+                        // pass 2 (rare after the first tiles; the insertion code exists once per chunk, not once per value)
+                        while (mask) {
+                            const int q = __ffs(mask) - 1; mask &= mask - 1;
+                            float sc = 0.f;
+#pragma unroll
+                            for (int z = 0; z < 32; ++z) if (z == q) sc = acc[4 * (c * 16 + (z >> 1)) + 2 * h + (z & 1)];
+                            const int col = colb + 8 * (c * 16 + (q >> 1)) + (q & 1);
+                            if (!(sc > kv[h] || (sc == kv[h] && col < ki[h]))) continue;          // the key may have risen meanwhile
+                            if (col >= P.n_to || (P.self_match && (long long)col == self_col)) continue;
+                            topk_insert<KMAX>(tv[h], ti[h], kv[h], ki[h], P.k, sc, (int)(P.to_base + col), P.to_base);
                         }
                     }
                 }
-                tc_fence_before();
-                mbar_arrive(tempty_bar(acc));
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
             }
-            if (row < P.n_from) {
+            // the four threads of a quad hold disjoint column sets of the same two rows: k rounds of "best head wins"
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
                 const size_t o = ((size_t)sp * P.n_from + row) * P.k;
 #pragma unroll
-                for (int z = 0; z < KMAX; ++z)
-                    if (z < P.k) { P.top_idx[o + z] = ti[z]; P.top_val[o + z] = ti[z] >= 0 ? (double)tv[z] : 0.0; }
-            }
-        }
-    }
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" :: "r"(tmem_base) : "memory");
-    }
-}
-
-// ---- 2-CTA variant (cta_group::2) -----------------------------------------------------------------------------------------
-// A CTA pair (cluster of 2, same TPC) computes M = 256 from-rows x N = 256 to-rows per MMA: each CTA stages ITS 128 rows of X
-// and ITS half (128 rows) of the Y tile, the leader CTA's single MMA thread issues tcgen05.mma.cta_group::2 reading both CTAs'
-// shared memory, and each CTA's TMEM receives the accumulators of its own 128 rows.  Per CTA and K step the L2 -> SM traffic is
-// 16 + 16 KB instead of 16 + 32 KB (the 1-CTA kernel streams 96 B/cycle/SM at full tensor rate and is L2->SM bound), which
-// also frees shared memory for 6 stages.  Barriers: `full` lives in the leader only (both CTAs' TMA complete_tx land there,
-// peer bit of the address cleared); `empty` / `tmem_full` exist per CTA and are signalled by multicast commits; `tmem_empty`
-// lives in the leader and collects the 2 x 128 epilogue threads (remote arrive from the peer).
-constexpr int D2STAGES = 6;
-constexpr int BH_BYTES = (DN / 2) * DK * 2;                           // this CTA's half of the Y tile: 16 KB
-constexpr unsigned PEER_MASK = 0xFEFFFFFFu;                          // clears the CTA-rank bit of a shared::cluster address
-
-__device__ __forceinline__ unsigned cluster_ctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(unsigned dst, const CUtensorMap *map, int c0, int c1, unsigned leader_bar) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 :: "r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(leader_bar) : "memory");
-}
-__device__ __forceinline__ void tc_commit_2sm(unsigned bar) {
-    asm volatile("{\n\t.reg .b16 m;\n\tmov.b16 m, 3;\n\t"
-                 "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], m;\n\t}" :: "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_2sm(unsigned d_tmem, uint64_t adesc, uint64_t bdesc, unsigned idesc, unsigned accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(unsigned local_bar) {      // arrive on the barrier at the same offset in CTA 0
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" :: "r"(local_bar & PEER_MASK) : "memory");
-}
-__device__ __forceinline__ unsigned umma_idesc_2sm() {                        // M = 256 (pair), N = 256
-    unsigned d = 0;
-    d |= 1u << 4; d |= 1u << 7; d |= 1u << 10;
-    d |= (unsigned)(DN >> 3) << 17;
-    d |= (unsigned)((2 * DM) >> 4) << 24;
-    return d;
-}
-
-template <int KMAX>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(DENSE_THREADS, 1)
-dense_cos_topk2_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y, const DenseParams P) {
-    extern __shared__ __align__(1024) unsigned char dsm_raw[];
-    unsigned char *dsm = dsm_raw + ((1024u - (s32(dsm_raw) & 1023u)) & 1023u);
-    unsigned char *sa = dsm;
-    unsigned char *sb = dsm + D2STAGES * A_BYTES;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(dsm + D2STAGES * (A_BYTES + BH_BYTES));
-    unsigned *tmem_slot = reinterpret_cast<unsigned *>(bars + 2 * D2STAGES + 4);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const unsigned rank = cluster_ctarank();
-    const unsigned bar0 = s32(bars);
-    auto full_bar = [&](int s) { return bar0 + 8u * s; };
-    auto empty_bar = [&](int s) { return bar0 + 8u * (D2STAGES + s); };
-    auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * D2STAGES + a); };
-    auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * D2STAGES + 2 + a); };
-
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < D2STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 256); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" :: "r"(s32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                                  // the peer's barriers are initialised before anything signals them
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
-
-    const int n_mpairs = (P.n_from + 2 * DM - 1) / (2 * DM);
-    const int n_units = n_mpairs * P.n_splits;
-    const int tiles_per = (P.n_ntiles + P.n_splits - 1) / P.n_splits;
-    const int n_kblk = (P.d + DK - 1) / DK;
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int stage = 0; unsigned phase = 0;
-            for (int u = pair; u < n_units; u += n_pairs) {
-                const int mp = u % n_mpairs, sp = u / n_mpairs;
-                const int t_lo = sp * tiles_per, t_hi = min(P.n_ntiles, t_lo + tiles_per);
-                for (int t = t_lo; t < t_hi; ++t) {
-                    for (int kb = 0; kb < n_kblk; ++kb) {
-                        mbar_wait(empty_bar(stage), phase ^ 1);
-                        if (rank == 0) mbar_expect_tx(full_bar(stage), 2 * (A_BYTES + BH_BYTES));
-                        tma_load_2d_2sm(s32(sa + stage * A_BYTES), &map_x, kb * DK, mp * 2 * DM + (int)rank * DM, full_bar(stage) & PEER_MASK);
-                        tma_load_2d_2sm(s32(sb + stage * BH_BYTES), &map_y, kb * DK, t * DN + (int)rank * (DN / 2), full_bar(stage) & PEER_MASK);
-                        if (++stage == D2STAGES) { stage = 0; phase ^= 1; }
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0 && rank == 0) {
-            const unsigned idesc = umma_idesc_2sm();
-            int stage = 0; unsigned phase = 0; int acc = 0; unsigned acc_phase = 0;
-            for (int u = pair; u < n_units; u += n_pairs) {
-                const int sp = u / n_mpairs;
-                const int t_lo = sp * tiles_per, t_hi = min(P.n_ntiles, t_lo + tiles_per);
-                for (int t = t_lo; t < t_hi; ++t) {
-                    mbar_wait(tempty_bar(acc), acc_phase ^ 1);            // both CTAs' epilogues drained this accumulator
-                    tc_fence_after();
-                    const unsigned d_tmem = tmem_base + (unsigned)(acc * DN);
-                    for (int kb = 0; kb < n_kblk; ++kb) {
-                        mbar_wait(full_bar(stage), phase);
-                        tc_fence_after();
-                        const uint64_t adesc = umma_desc(s32(sa + stage * A_BYTES));
-                        const uint64_t bdesc = umma_desc(s32(sb + stage * BH_BYTES));
+                for (int z = 0; z < KMAX; ++z) {
+                    if (z < P.k) {
+                        float bv = tv[h][0]; int bi = ti[h][0];
 #pragma unroll
-                        for (int kk = 0; kk < DK / UMMA_K; ++kk)
-                            tc_mma_2sm(d_tmem, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), idesc, (kb | kk) ? 1u : 0u);
-                        tc_commit_2sm(empty_bar(stage));                  // frees the stage in BOTH CTAs
-                        if (++stage == D2STAGES) { stage = 0; phase ^= 1; }
-                    }
-                    tc_commit_2sm(tfull_bar(acc));                        // accumulators complete in both CTAs
-                    if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp >= 4) {
-        const int ew = warp - 4;
-        const int row_in_blk = ew * 32 + lane;
-        int acc = 0; unsigned acc_phase = 0;
-        for (int u = pair; u < n_units; u += n_pairs) {
-            const int mp = u % n_mpairs, sp = u / n_mpairs;
-            const int t_lo = sp * tiles_per, t_hi = min(P.n_ntiles, t_lo + tiles_per);
-            const int row = mp * 2 * DM + (int)rank * DM + row_in_blk;
-            const long long self_col = P.from_base + row - P.to_base;
-            float tv[KMAX]; int ti[KMAX];
-#pragma unroll
-            for (int q = 0; q < KMAX; ++q) { tv[q] = P.min_sim; ti[q] = -1; }
-            float kv = P.min_sim; int ki = -1;
-            for (int t = t_lo; t < t_hi; ++t) {
-                mbar_wait(tfull_bar(acc), acc_phase);
-                tc_fence_after();
-                const unsigned taddr = tmem_base + ((unsigned)(ew * 32) << 16) + (unsigned)(acc * DN);
-                for (int c0 = 0; c0 < DN; c0 += 32) {
-                    unsigned r[32];
-                    tmem_ld32(taddr + (unsigned)c0, r);
-                    const int colb = t * DN + c0;
-                    unsigned mask = 0u;
-#pragma unroll
-                    for (int q = 0; q < 32; ++q) {
-                        const float sc = __uint_as_float(r[q]);
-                        if (sc > kv || (sc == kv && colb + q < ki)) mask |= 1u << q;
-                    }
-                    while (mask) {
-                        const int q = __ffs(mask) - 1; mask &= mask - 1;
-                        float sc = 0.f;
-#pragma unroll
-                        for (int z = 0; z < 32; ++z) if (z == q) sc = __uint_as_float(r[z]);
-                        const int col = colb + q;
-                        if (!(sc > kv || (sc == kv && col < ki))) continue;
-                        if (col >= P.n_to || (P.self_match && (long long)col == self_col)) continue;
-                        float cv = sc; int ci = (int)(P.to_base + col);
-#pragma unroll
-                        for (int z = 0; z < KMAX; ++z) {
-                            if (z < P.k) {
-                                const bool before = cv > tv[z] || (cv == tv[z] && (ti[z] < 0 || ci < ti[z]));
-                                if (before) { const float fv = tv[z]; const int fi = ti[z]; tv[z] = cv; ti[z] = ci; cv = fv; ci = fi; }
-                                if (z == P.k - 1) { kv = tv[z]; ki = ti[z] < 0 ? -1 : ti[z] - (int)P.to_base; }
-                            }
+                        for (int m = 1; m <= 2; m <<= 1) {
+                            const float ov = __shfl_xor_sync(FULL, bv, m); const int oi = __shfl_xor_sync(FULL, bi, m);
+                            if (oi >= 0 && (bi < 0 || ov > bv || (ov == bv && oi < bi))) { bv = ov; bi = oi; }
                         }
+                        if (bi >= 0 && ti[h][0] == bi) {
+#pragma unroll
+                            for (int w = 0; w + 1 < KMAX; ++w) { tv[h][w] = tv[h][w + 1]; ti[h][w] = ti[h][w + 1]; }
+                            tv[h][KMAX - 1] = P.min_sim; ti[h][KMAX - 1] = -1;
+                        }
+                        if (q4 == 0 && row < P.n_from) { P.top_idx[o + z] = bi; P.top_val[o + z] = bi >= 0 ? (double)bv : 0.0; }
                     }
                 }
-                tc_fence_before();
-                mbar_arrive_leader(tempty_bar(acc));
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-            if (row < P.n_from) {
-                const size_t o = ((size_t)sp * P.n_from + row) * P.k;
-#pragma unroll
-                for (int z = 0; z < KMAX; ++z)
-                    if (z < P.k) { P.top_idx[o + z] = ti[z]; P.top_val[o + z] = ti[z] >= 0 ? (double)tv[z] : 0.0; }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                                  // neither CTA frees TMEM while the pair still computes
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" :: "r"(tmem_base) : "memory");
-    }
+    if (MCAST) cluster_sync_all();                                       // no CTA exits while its peer may still write into it
 }
 
 // rows -> l2-normalised bf16 (fp64 or fp32 in); zero rows stay zero.  One warp per row.
@@ -455,6 +298,25 @@ static int make_map(EncodeTiledFn enc, CUtensorMap *m, const void *base, int n_r
     return 0;
 }
 
+template <int KMAX, bool MCAST>
+static int dense_launch(EncodeTiledFn enc, const void *x_bf16, const void *y_bf16, DenseParams P, int sms, cudaStream_t st) {
+    CUtensorMap mx, my;
+    if (make_map(enc, &mx, x_bf16, P.n_from, P.d, DM)) return 1;
+    if (make_map(enc, &my, y_bf16, P.n_to, P.d, MCAST ? DN / 2 : DN)) return 1;
+    const int G = MCAST ? 2 : 1;
+    int units = (P.n_mblocks + G - 1) / G * P.n_splits; if (units > sms / G) units = sms / G;
+    auto kern = dense_cos_topk_kernel<KMAX, MCAST>;
+    PFZ_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DENSE_SMEM));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(G * units)); cfg.blockDim = dim3(DENSE_THREADS); cfg.dynamicSmemBytes = DENSE_SMEM; cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = G; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    PFZ_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, mx, my, P));
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
 }  // namespace pfz
 
 using namespace pfz;
@@ -465,7 +327,7 @@ int pfz_rows_to_bf16(const void *x, int32_t is_f64, int64_t ld, int32_t n_rows, 
                      void *stream) {
     if (n_rows <= 0) return 0;
     PFZ_REQUIRE(d_pad >= d && d_pad % 8 == 0, "pfz_rows_to_bf16: d_pad %d must be >= d and a multiple of 8", d_pad);
-    int grid = (n_rows + 7) / 8; if (grid > 148 * 16) grid = 148 * 16;
+    int grid = (n_rows + 7) / 8; if (grid > SM_COUNT * 16) grid = SM_COUNT * 16;
     if (is_f64) rows_normalize_bf16_kernel<double><<<grid, 256, 0, as_stream(stream)>>>((const double *)x, ld, n_rows, d, d_pad, normalize, (__nv_bfloat16 *)out_bf16);
     else        rows_normalize_bf16_kernel<float><<<grid, 256, 0, as_stream(stream)>>>((const float *)x, ld, n_rows, d, d_pad, normalize, (__nv_bfloat16 *)out_bf16);
     PFZ_LAUNCH_OK();
@@ -480,7 +342,6 @@ int pfz_dense_cos_topk(const void *x_bf16, const void *y_bf16, int32_t n_from, i
     PFZ_REQUIRE(((uintptr_t)x_bf16 % 16) == 0 && ((uintptr_t)y_bf16 % 16) == 0, "pfz_dense_cos_topk: operands must be 16-byte aligned");
     if (n_from <= 0) return 0;
     PFZ_REQUIRE(n_to > 0, "pfz_dense_cos_topk: empty to-matrix");
-    cudaStream_t st = as_stream(stream);
     static EncodeTiledFn enc = nullptr;
     if (!enc) {
         void *fn = nullptr; cudaDriverEntryPointQueryResult qres;
@@ -488,11 +349,8 @@ int pfz_dense_cos_topk(const void *x_bf16, const void *y_bf16, int32_t n_from, i
         PFZ_REQUIRE(fn && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available in this driver");
         enc = (EncodeTiledFn)fn;
     }
-    const char *env2 = getenv("PFZ_K4_2CTA");                   // cta_group::2 variant (CTA pairs, half the to-operand traffic per SM): the
-    const bool two_cta = env2 ? atoi(env2) != 0 : true;         // default since it was validated on hardware (13.66 vs 14.04 ms at 100k x 100k x 768); 0 = single-CTA kernel
-    CUtensorMap mx, my;
-    if (make_map(enc, &mx, x_bf16, n_from, d, DM)) return 1;
-    if (make_map(enc, &my, y_bf16, n_to, d, two_cta ? DN / 2 : DN)) return 1;
+    const char *env2 = getenv("PFZ_K4_2CTA");                   // CTA pairs sharing the to-tile through TMA multicast (half the to-operand
+    const bool two_cta = env2 ? atoi(env2) != 0 : true;         // traffic per SM); 0 = one CTA per row block
     DenseParams P;
     P.n_from = n_from; P.n_to = n_to; P.d = d; P.k = k; P.min_sim = (float)min_similarity; P.self_match = self_match;
     P.from_base = from_index_base; P.to_base = to_index_base;
@@ -502,30 +360,12 @@ int pfz_dense_cos_topk(const void *x_bf16, const void *y_bf16, int32_t n_from, i
     int dev = 0, sms = 0;
     PFZ_CUDA_OK(cudaGetDevice(&dev));
     PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    if (two_cta) {
-        const size_t smem2 = (size_t)D2STAGES * (A_BYTES + BH_BYTES) + (2 * D2STAGES + 4) * 8 + 16 + 1024;
-        const int n_mpairs = (n_from + 2 * DM - 1) / (2 * DM);
-        int pairs = n_mpairs * n_splits; if (pairs > sms / 2) pairs = sms / 2;
-#define PFZ_DENSE2_LAUNCH(KM)                                                                                                 \
-    do {                                                                                                                      \
-        PFZ_CUDA_OK(cudaFuncSetAttribute(dense_cos_topk2_kernel<KM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2)); \
-        dense_cos_topk2_kernel<KM><<<2 * pairs, DENSE_THREADS, smem2, st>>>(mx, my, P);                                        \
-    } while (0)
-        if (k <= 4) PFZ_DENSE2_LAUNCH(4); else if (k <= 10) PFZ_DENSE2_LAUNCH(10); else if (k <= 16) PFZ_DENSE2_LAUNCH(16); else PFZ_DENSE2_LAUNCH(32);
-#undef PFZ_DENSE2_LAUNCH
-        PFZ_LAUNCH_OK();
-        return 0;
-    }
-    const size_t smem = (size_t)DSTAGES * (A_BYTES + B_BYTES) + (2 * DSTAGES + 4) * 8 + 16 + 1024;
-    int grid = P.n_mblocks * n_splits; if (grid > sms) grid = sms;
-#define PFZ_DENSE_LAUNCH(KM)                                                                                                \
-    do {                                                                                                                    \
-        PFZ_CUDA_OK(cudaFuncSetAttribute(dense_cos_topk_kernel<KM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        dense_cos_topk_kernel<KM><<<grid, DENSE_THREADS, smem, st>>>(mx, my, P);                                             \
-    } while (0)
-    if (k <= 4) PFZ_DENSE_LAUNCH(4); else if (k <= 10) PFZ_DENSE_LAUNCH(10); else if (k <= 16) PFZ_DENSE_LAUNCH(16); else PFZ_DENSE_LAUNCH(32);
+    cudaStream_t st = as_stream(stream);
+#define PFZ_DENSE_LAUNCH(KM) (two_cta ? dense_launch<KM, true>(enc, x_bf16, y_bf16, P, sms, st) : dense_launch<KM, false>(enc, x_bf16, y_bf16, P, sms, st))
+    if (k <= 4) return PFZ_DENSE_LAUNCH(4);
+    if (k <= 10) return PFZ_DENSE_LAUNCH(10);
+    if (k <= 16) return PFZ_DENSE_LAUNCH(16);
+    return PFZ_DENSE_LAUNCH(32);
 #undef PFZ_DENSE_LAUNCH
-    PFZ_LAUNCH_OK();
-    return 0;
 }
 }

@@ -266,7 +266,7 @@ int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32
                  const int64_t *grp_word_off, uint32_t *packed, int32_t *slen, void *stream) {
     if (n_to <= 0) return 0;
     const int n_grp = (n_to + 31) / 32;
-    int grid = (n_grp + 7) / 8; if (grid > 148 * 8) grid = 148 * 8;
+    int grid = (n_grp + 7) / 8; if (grid > SM_COUNT * 8) grid = SM_COUNT * 8;
     lev_pack_kernel<<<grid, 256, 0, as_stream(stream)>>>(to_blob, to_offsets, order, n_to, sym_table, grp_word_off, packed, slen);
     PFZ_LAUNCH_OK();
     return 0;
@@ -306,7 +306,7 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits, int32_t n_from,
                   int32_t *best_idx, double *best_score, int32_t *best_dist, void *stream) {
     if (n_from <= 0) return 0;
-    int grid = (n_from + 255) / 256; if (grid > 148 * 8) grid = 148 * 8;
+    int grid = (n_from + 255) / 256; if (grid > SM_COUNT * 8) grid = SM_COUNT * 8;
     lev_merge_kernel<<<grid, 256, 0, as_stream(stream)>>>(part_idx, part_score, part_dist, n_splits, n_from, best_idx, best_score, best_dist);
     PFZ_LAUNCH_OK();
     return 0;

@@ -331,8 +331,8 @@ __device__ __forceinline__ float float_floor(double x) {
     return f;
 }
 
-// Register caps measured on B200 (100k x 100k): the mixed-precision kernel is fastest at 64 registers (16 blocks of
-// 2 warps per SM, a few spilled bytes), the fp64 kernel at 80 (12 blocks); fewer registers spill into the hot loop.
+// Register caps (inherited, not re-tuned on H100): the mixed-precision kernel at 64 registers (16 blocks of 2 warps per
+// SM, a few spilled bytes), the fp64 kernel at 80 (12 blocks); fewer registers spill into the hot loop.
 template <int WARPS, int D, bool APPROX, bool PRUNE>
 __global__ void __launch_bounds__(WARPS * 32, (APPROX && !PRUNE && D <= 4) ? 16 : 12) spcos_dense_kernel(const SpcosParams P) {
     extern __shared__ __align__(16) unsigned char dyn[];
@@ -740,25 +740,25 @@ int pfz_index_build(const int32_t *indptr, const int32_t *indices, const double 
     void *sws = reinterpret_cast<char *>(ws) + ((((size_t)ncell + 1) * 4 + 255) / 256) * 256;
     PFZ_CUDA_OK(cudaMemsetAsync(seg, 0, ((size_t)ncell + 1) * 4, st));
     if (n_rows > 0) {
-        index_count_kernel<<<grid_for2((int64_t)n_rows * 32, 256, 148 * 16), 256, 0, st>>>(indptr, indices, n_rows, tile, n_tiles, seg);
+        index_count_kernel<<<grid_for2((int64_t)n_rows * 32, 256, SM_COUNT * 16), 256, 0, st>>>(indptr, indices, n_rows, tile, n_tiles, seg);
         PFZ_LAUNCH_OK();
     }
     if (scan_exclusive_i32(seg, seg, ncell + 1, sws, st)) return 1;
     if (n_rows > 0) {
         PFZ_CUDA_OK(cudaMemsetAsync(cur, 0, ((size_t)ncell + 1) * 4, st));
         if (term_maxw) PFZ_CUDA_OK(cudaMemsetAsync(term_maxw, 0, (size_t)n_vocab * 4, st));
-        index_fill_kernel<<<grid_for2((int64_t)n_rows * 32, 256, 148 * 16), 256, 0, st>>>(indptr, indices, data, n_rows, tile, n_tiles, seg, cur,
+        index_fill_kernel<<<grid_for2((int64_t)n_rows * 32, 256, SM_COUNT * 16), 256, 0, st>>>(indptr, indices, data, n_rows, tile, n_tiles, seg, cur,
                                                                                             post_idx, post_val, reinterpret_cast<int *>(term_maxw));
         PFZ_LAUNCH_OK();
         if (flags & PFZ_INDEX_BANK_ORDER32) {
-            index_bank_order_kernel<32><<<grid_for2(ncell, 128, 148 * 16), 128, 0, st>>>(seg, ncell, post_idx, post_val);
+            index_bank_order_kernel<32><<<grid_for2(ncell, 128, SM_COUNT * 16), 128, 0, st>>>(seg, ncell, post_idx, post_val);
             PFZ_LAUNCH_OK();
         } else if (flags & PFZ_INDEX_BANK_ORDER) {
-            index_bank_order_kernel<16><<<grid_for2(ncell, 128, 148 * 16), 128, 0, st>>>(seg, ncell, post_idx, post_val);
+            index_bank_order_kernel<16><<<grid_for2(ncell, 128, SM_COUNT * 16), 128, 0, st>>>(seg, ncell, post_idx, post_val);
             PFZ_LAUNCH_OK();
         }
         if (post_val32) {                                       // fp32 copy of the weights for the mixed-precision filter
-            to_f32_kernel<<<148 * 8, 256, 0, st>>>(post_val, 0, seg + ncell, post_val32);
+            to_f32_kernel<<<SM_COUNT * 8, 256, 0, st>>>(post_val, 0, seg + ncell, post_val32);
             PFZ_LAUNCH_OK();
         }
     }
@@ -829,7 +829,7 @@ int pfz_topk_merge(const int32_t *idx, const double *val, int32_t n_lists, int32
     PFZ_REQUIRE(k_out >= 1 && k_out <= 32, "pfz_topk_merge: k_out=%d unsupported (1..32)", k_out);
     PFZ_REQUIRE(n_lists >= 1 && k_in >= 1, "pfz_topk_merge: bad n_lists/k_in");
     if (n_from <= 0) return 0;
-    topk_merge_kernel<<<grid_for2((int64_t)n_from * 32, 256, 148 * 16), 256, 0, as_stream(stream)>>>(idx, val, n_lists, n_from, k_in, k_out, out_idx, out_val);
+    topk_merge_kernel<<<grid_for2((int64_t)n_from * 32, 256, SM_COUNT * 16), 256, 0, as_stream(stream)>>>(idx, val, n_lists, n_from, k_in, k_out, out_idx, out_val);
     PFZ_LAUNCH_OK();
     return 0;
 }

@@ -6,17 +6,16 @@
 // post-processing (polyfuzz/models/_utils.py:84-91, 128-146), like the other K2 variants (pfz_spcos.cu); results are
 // bit-identical to them (same exact fp64 re-scoring, same ranking key).
 //
-// Why: ncu on the per-row kernels (profiles/k2_r01_bench_metrics.txt) showed them bound by instruction issue -- ~93
-// warp instructions per 32 postings, most of it fetching postings and per-(row, tile) bookkeeping.  On name-like
+// Why: the per-row kernels are bound by instruction issue -- most of it fetching postings and per-(row, tile)
+// bookkeeping.  On name-like
 // data a few hundred n-grams carry > 90 % of the postings ("inc", "llc", "cor", ...), so from-rows share their heavy
 // terms.  Here
 //   * from-rows are CLUSTERED by their three heaviest terms (sort of a 64-bit key), so a block of consecutive rows
 //     shares most heavy terms (company names: one posting load serves ~4 of 8 rows on average);
 //   * a block table (per block: distinct terms, per term the list of (row-in-block, weight)) is built once per call;
 //   * accumulators acc[BF][tile] are FIXED-POINT sums in shared memory, updated with red.shared.add.u32: a
-//     fire-and-forget integer atomic that retires at one warp-update per SM-cycle on B200
-//     (profiles/atoms_probe_r02.txt; a ld/fma/st read-modify-write chain managed 4.3 cycles with 8 warps and 33 with
-//     one; float and 64-bit shared-memory adds are CAS loops).  Integer adds are associative, so the warps of the CTA share
+//     fire-and-forget integer atomic (a ld/fma/st read-modify-write chain serialises on the latency of each update;
+//     float and 64-bit shared-memory adds are CAS loops).  Integer adds are associative, so the warps of the CTA share
 //     one accumulator tile and consume the unit's work items (<= 32 postings of one term each) in any order, with no
 //     hazards and no ordering.  Default: two 16-bit accumulators per word (unit 2^-15, to-rows j and j + tile/2 share
 //     word j) -- twice the tile in the same shared memory; 32-bit accumulators (unit 2^-26) remain selectable;
@@ -247,9 +246,8 @@ __device__ __forceinline__ unsigned warp_sort_desc_u32(unsigned x, int lane) {
 }
 
 // ---- main kernel (version 3) -----------------------------------------------------------------------------------
-// Laid out for instruction count and registers after the ncu profile of version 2 (one monolithic kernel;
-// profiles/k2_r02_block_v2_metrics.txt: 67 warp instructions per work item, 43 per 256 scanned cells, local-memory spills in
-// both loops, 5 barriers per (block, tile) unit):
+// Laid out for instruction count and registers (a monolithic version spilled to local memory in both loops and needed
+// 5 barriers per (block, tile) unit):
 //   * everything rare -- queueing candidates, maintaining the K largest sums, exact re-scoring, the top-k list -- lives in
 //     NOINLINE functions whose state is in shared memory (B3Row), so the two hot loops (work items, scan) keep a handful of
 //     registers and nothing spills;
@@ -918,14 +916,14 @@ int64_t pfz_spcos_block_ws_bytes(int32_t n_from, int64_t nnz_cap_from, int32_t n
 }
 
 int pfz_index_pack_q26(const uint16_t *post_idx, const double *post_val, const int32_t *nnz_dev, void *post_pk, void *stream) {
-    blk_pack_kernel<<<148 * 8, 256, 0, as_stream(stream)>>>(post_idx, post_val, nnz_dev, reinterpret_cast<uint2 *>(post_pk));
+    blk_pack_kernel<<<SM_COUNT * 8, 256, 0, as_stream(stream)>>>(post_idx, post_val, nnz_dev, reinterpret_cast<uint2 *>(post_pk));
     PFZ_LAUNCH_OK();
     return 0;
 }
 
 int pfz_index_pack_q15(const uint16_t *post_idx, const double *post_val, const int32_t *nnz_dev, int32_t tile, void *post_pk, void *stream) {
     PFZ_REQUIRE(tile >= 256 && tile <= 8192 && (tile % 256) == 0, "pfz_index_pack_q15: tile %d must be a multiple of 256 in 256..8192", tile);
-    blk_pack15_kernel<<<148 * 8, 256, 0, as_stream(stream)>>>(post_idx, post_val, nnz_dev, tile / 2, reinterpret_cast<uint2 *>(post_pk));
+    blk_pack15_kernel<<<SM_COUNT * 8, 256, 0, as_stream(stream)>>>(post_idx, post_val, nnz_dev, tile / 2, reinterpret_cast<uint2 *>(post_pk));
     PFZ_LAUNCH_OK();
     return 0;
 }
@@ -963,26 +961,26 @@ int pfz_spcos_topk_block(const int32_t *a_indptr, const int32_t *a_indices, cons
     const int64_t vp = pow2_at_least(n_vocab), np = pow2_at_least(n_from);
     const int n_groups = (n_from + block_rows - 1) / block_rows;
 
-    blk_term_key_kernel<<<blk_grid(vp, 256, 148 * 8), 256, 0, st>>>(seg, n_vocab, n_tiles, term_keys, vp);
+    blk_term_key_kernel<<<blk_grid(vp, 256, SM_COUNT * 8), 256, 0, st>>>(seg, n_vocab, n_tiles, term_keys, vp);
     PFZ_LAUNCH_OK();
     if (pfz_sort_u64(term_keys, vp, stream)) return 1;
-    blk_term_rank_kernel<<<blk_grid(n_vocab, 256, 148 * 8), 256, 0, st>>>(term_keys, n_vocab, term_rank);
+    blk_term_rank_kernel<<<blk_grid(n_vocab, 256, SM_COUNT * 8), 256, 0, st>>>(term_keys, n_vocab, term_rank);
     PFZ_LAUNCH_OK();
-    blk_row_key_kernel<<<blk_grid(np, 256, 148 * 16), 256, 0, st>>>(a_indptr, a_indices, term_rank, n_from, row_keys, np);
+    blk_row_key_kernel<<<blk_grid(np, 256, SM_COUNT * 16), 256, 0, st>>>(a_indptr, a_indices, term_rank, n_from, row_keys, np);
     PFZ_LAUNCH_OK();
     if (pfz_sort_u64(row_keys, np, stream)) return 1;
-    blk_perm_kernel<<<blk_grid(n_from + 1, 256, 148 * 16), 256, 0, st>>>(row_keys, a_indptr, n_from, perm, pos_ptr);
+    blk_perm_kernel<<<blk_grid(n_from + 1, 256, SM_COUNT * 16), 256, 0, st>>>(row_keys, a_indptr, n_from, perm, pos_ptr);
     PFZ_LAUNCH_OK();
     if (scan_exclusive_i32(pos_ptr, pos_ptr, (int64_t)n_from + 1, w + L.scan_ws, st)) return 1;
     const int row_stride = tile * (acc_bits == 16 ? 2 : 4) + 128;  // 32 dump words behind every row's cells
     if (block_rows == 4)
-        blk_table_kernel<4><<<blk_grid((int64_t)n_groups * 32, 128, 148 * 16), 128, 0, st>>>(a_indptr, a_indices, a_data, n_from, perm, pos_ptr, row_stride,
+        blk_table_kernel<4><<<blk_grid((int64_t)n_groups * 32, 128, SM_COUNT * 16), 128, 0, st>>>(a_indptr, a_indices, a_data, n_from, perm, pos_ptr, row_stride,
                                                                                              blk_terms, blk_fvdesc, blk_fv, descs, n_groups, err_flag_dev);
     else if (block_rows == 8)
-        blk_table_kernel<8><<<blk_grid((int64_t)n_groups * 32, 128, 148 * 16), 128, 0, st>>>(a_indptr, a_indices, a_data, n_from, perm, pos_ptr, row_stride,
+        blk_table_kernel<8><<<blk_grid((int64_t)n_groups * 32, 128, SM_COUNT * 16), 128, 0, st>>>(a_indptr, a_indices, a_data, n_from, perm, pos_ptr, row_stride,
                                                                                              blk_terms, blk_fvdesc, blk_fv, descs, n_groups, err_flag_dev);
     else
-        blk_table_kernel<16><<<blk_grid((int64_t)n_groups * 32, 64, 148 * 16), 128, 0, st>>>(a_indptr, a_indices, a_data, n_from, perm, pos_ptr, row_stride,
+        blk_table_kernel<16><<<blk_grid((int64_t)n_groups * 32, 64, SM_COUNT * 16), 128, 0, st>>>(a_indptr, a_indices, a_data, n_from, perm, pos_ptr, row_stride,
                                                                                               blk_terms, blk_fvdesc, blk_fv, descs, n_groups, err_flag_dev);
     PFZ_LAUNCH_OK();
     PFZ_CUDA_OK(cudaMemsetAsync(counters, 0, sizeof(int32_t) * (size_t)n_splits, st));

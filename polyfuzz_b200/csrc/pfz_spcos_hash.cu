@@ -6,7 +6,7 @@
 //
 // Why: on sparse inputs (BASELINE configs[4]: uniform 8..32-character strings, 0.006 postings per scored pair) a from-row
 // touches ~6 000 of 1 000 000 to-rows.  The tile-based kernels pay per (from-row, to-tile) unit -- 1 954 tiles x 17
-// segment look-ups per row for a handful of postings each: 805 ms at 1M x 1M on one B200 (profiles/bench_n1_r02_baseline.json).
+// segment look-ups per row for a handful of postings each.
 // Here the work is proportional to the postings: the index is tiled as coarsely as its 16-bit local rows allow (65 536 rows),
 // the CTA walks the row's (term, tile) segments once, and every posting is one hash insert (atom.shared.cas) plus one
 // fire-and-forget fixed-point add (red.shared.add.u32, unit 2^-26, see pfz_spcos_block.cu).  The table then is scanned
@@ -86,7 +86,7 @@ __host__ __device__ inline size_t hash_arena_bytes() {
 }
 
 #ifndef PFZ_HASH_MIN_CTAS
-#define PFZ_HASH_MIN_CTAS 8    // 64 registers per thread: without the bound ptxas spends 119 and 4 CTAs fit (22.6 vs 14.2 ms)
+#define PFZ_HASH_MIN_CTAS 8    // 64 registers per thread: without the bound ptxas spends 119 and only 4 CTAs fit
 #endif
 template <int H, int LOGH>
 __global__ void __launch_bounds__(HASH_NT, PFZ_HASH_MIN_CTAS) spcos_hash_kernel(const HashParams P) {

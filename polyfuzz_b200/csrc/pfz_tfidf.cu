@@ -1,4 +1,4 @@
-// pfz_tfidf.cu -- K1: character n-gram TF-IDF vectoriser on sm_100a.
+// pfz_tfidf.cu -- K1: character n-gram TF-IDF vectoriser on sm_90a.
 //
 // Replaces the reference's per-string Python loops (polyfuzz/models/_tfidf.py:120-146) and the
 // scikit-learn vocabulary / tf-idf / l2 arithmetic they feed (sk:feature_extraction/text.py:1257-1320,
@@ -404,7 +404,7 @@ __global__ void __launch_bounds__(256) emit_write_kernel(const uint64_t *__restr
     }
 }
 
-static int grid_for(int64_t work_items, int threads, int cap = 148 * 16) {
+static int grid_for(int64_t work_items, int threads, int cap = SM_COUNT * 16) {
     int64_t g = (work_items + threads - 1) / threads;
     if (g < 1) g = 1;
     if (g > cap) g = cap;
@@ -437,7 +437,7 @@ int pfz_ngram_rows(const uint32_t *blob, const int64_t *offsets, int32_t n_rows,
     if (n_rows <= 0) return 0;
     const int rs = (flags & PFZ_FLAG_REMOVE_SPACE) ? 1 : 0;
     cudaStream_t st = as_stream(stream);
-    int grid = grid_for((int64_t)n_rows * 32, 256, 148 * 8);
+    int grid = grid_for((int64_t)n_rows * 32, 256, SM_COUNT * 8);
     if (clean) ngram_rows_warp_kernel<true><<<grid, 256, 0, st>>>(blob, offsets, n_rows, lo, hi, rs, sym_table, base, occ_ptr, codes, tf, row_cnt);
     else       ngram_rows_warp_kernel<false><<<grid, 256, 0, st>>>(blob, offsets, n_rows, lo, hi, rs, sym_table, base, occ_ptr, codes, tf, row_cnt);
     PFZ_LAUNCH_OK();
@@ -502,7 +502,7 @@ int pfz_sort_u64(uint64_t *keys, int64_t n, void *stream) {
     for (int64_t k = (int64_t)BS_TILE * 2; k <= n; k <<= 1) {
         int64_t j = k >> 1;
         for (; j >= BS_TILE; j >>= 1) {
-            bitonic_global_kernel<<<grid_for(n >> 1, 256, 148 * 32), 256, 0, st>>>(keys, n, k, j);
+            bitonic_global_kernel<<<grid_for(n >> 1, 256, SM_COUNT * 32), 256, 0, st>>>(keys, n, k, j);
             PFZ_LAUNCH_OK();
         }
         bitonic_local_kernel<<<(unsigned)nblk, BS_THREADS, 0, st>>>(keys, n, k, k, j);

@@ -1,13 +1,13 @@
 """K4 host driver: dense cosine top-k of pre-computed embeddings on the tensor cores (include/pfz.h,
 pfz_rows_to_bf16 + pfz_dense_cos_topk).  Inputs are rounded to bf16 (after l2 normalisation in fp32);
-products accumulate in fp32 in TMEM; the ranking key is (score desc, index asc) on those fp32 values."""
+products accumulate in fp32 (wgmma register accumulators); the ranking key is (score desc, index asc) on those fp32 values."""
 import numpy as np
 import torch
 
 from . import _lib
 from .engine import _dev, _p, _stream, topk_merge
 
-SM_COUNT = 148
+SM_COUNT = 132                     # H100 SXM
 
 
 def to_bf16_rows(x, normalize=True):
@@ -43,7 +43,7 @@ def dense_topk(x_bf16, y_bf16, k, min_similarity=0.0, self_match=False, from_ind
     if n_from == 0:
         return torch.empty((0, k), dtype=torch.int32, device=dev), torch.empty((0, k), dtype=torch.float64, device=dev)
     n_mblocks = (n_from + 127) // 128
-    n_ntiles = (n_to + 255) // 256
+    n_ntiles = (n_to + 127) // 128                     # 128-wide to-tiles (pfz_dense.cu DN)
     if n_splits is None:
         n_splits = max(1, min(n_ntiles, (2 * SM_COUNT + n_mblocks - 1) // n_mblocks))
     n_splits = max(1, min(int(n_splits), n_ntiles))

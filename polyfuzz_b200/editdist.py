@@ -123,7 +123,7 @@ class EditTargets:
 
 def default_splits(n_from, n_grp):
     # ~4 (pattern, to-split) tasks per resident warp: patterns differ in length, finer tasks balance the tail
-    want = 4 * 148 * 48
+    want = 4 * 132 * 48
     return max(1, min(n_grp, (want + max(n_from, 1) - 1) // max(n_from, 1)))
 
 

@@ -25,7 +25,7 @@ N_CODE_POINTS = 0x110000
 
 def _dev():
     if not torch.cuda.is_available():
-        raise RuntimeError("polyfuzz_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("polyfuzz_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 
 
@@ -166,7 +166,7 @@ class _Rows:
 
 
 class NgramTfidf:
-    """B200 statement of `TfidfVectorizer(min_df=1, analyzer=TFIDF._create_ngrams)` as the reference
+    """GPU statement of `TfidfVectorizer(min_df=1, analyzer=TFIDF._create_ngrams)` as the reference
     uses it (polyfuzz/models/_tfidf.py:102-118).  fit() learns vocabulary (alphabetical == ascending
     n-gram code) and idf; transform() emits the l2-normalised CSR in HBM."""
 
@@ -497,7 +497,7 @@ def choose_variant(density, max_row_nnz=None, n_to=None):
     return DENSE_VARIANT
 
 
-def _auto_splits(n_from, n_tiles, sm_count=148):
+def _auto_splits(n_from, n_tiles, sm_count=132):
     want = sm_count * 32                                   # enough (from-row, tile-range) tasks to fill every SM
     if n_from >= want:
         return 1
@@ -513,8 +513,8 @@ HASH_SLOTS = int(os.environ.get("PFZ_HASH_SLOTS", "0"))          # 0 = choose fr
 
 
 def _hash_slots(index):
-    """Table size of the hash kernel.  2 048 slots (16 KB, 8 CTAs per SM) measured fastest on the 1M x 1M uniform strings
-    (18.0 ms per 100 000 from-rows against 20.4 / 44.0 ms with 8 192 / 16 384 slots): rows that visit more postings take more
+    """Table size of the hash kernel.  2 048 slots (16 KB, 8 CTAs per SM; inherited, not re-tuned on H100) beat 8 192 and
+    16 384 on the 1M x 1M uniform strings: rows that visit more postings take more
     passes over tile ranges, and a pass whose table fills is redone over halved to-row ranges inside the kernel."""
     return HASH_SLOTS if HASH_SLOTS else 2048
 BLOCK_MAX_ROWS = (1 << 22) - 1                                   # row id field of the block kernel's clustering key

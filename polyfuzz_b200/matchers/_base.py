@@ -1,7 +1,7 @@
 """The plugin type.
 
 When the reference package is importable at import time its own `polyfuzz.models.BaseMatcher` is the base
-class, so the B200 matchers ARE reference plugins.  Otherwise an identical ABC is defined here (mirror of
+class, so this package's matchers ARE reference plugins.  Otherwise an identical ABC is defined here (mirror of
 polyfuzz/models/_base.py:6-31: abstract match(), attributes model_id and type) and, should `polyfuzz`
 become importable later in the process, every matcher class is registered with the reference's ABC as a
 virtual subclass -- either way `isinstance(m, polyfuzz.models.BaseMatcher)` holds and

@@ -1,5 +1,5 @@
 """TFIDF matcher -- drop-in for polyfuzz.models.TFIDF (polyfuzz/models/_tfidf.py:11-146) running the
-vectoriser (K1) and the sparse cosine top-n (K2) on a B200."""
+vectoriser (K1) and the sparse cosine top-n (K2) on an H100."""
 from typing import List, Tuple
 
 import numpy as np

@@ -10,18 +10,18 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_sessionstart(session):
     """Built artefacts are git-ignored: (re)build the C-ABI library, the host packer and the CPU oracle when they are
-    missing or older than their sources (no-op on the GPU box, where the snapshot already carries them)."""
+    missing or older than their sources (a no-op when build() already made them)."""
     from polyfuzz_b200 import build as b
     from oracle import native
     native.build()                                          # gcc only
     b.build_hostpack()                                      # gcc only
     try:
-        b.build(force=False)                                # nvcc (cross-compiles sm_100a without a GPU)
+        b.build(force=False)                                # nvcc (cross-compiles sm_90a without a GPU)
     except (RuntimeError, OSError) as e:
         import torch
         if torch.cuda.is_available() or "gpu" in (session.config.getoption("-m") or ""):

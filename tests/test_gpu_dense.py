@@ -1,4 +1,4 @@
-"""GPU tests of K4 (dense bf16 tcgen05 cosine top-k) against an fp64 reference computed from the SAME
+"""GPU tests of K4 (dense bf16 wgmma cosine top-k) against an fp64 reference computed from the SAME
 bf16-rounded inputs.  Tolerance (north_star): scores within 1e-5; indices must be an exact top-k of the fp64
 scores up to that tolerance (every returned score >= k-th fp64 score - 2e-5, ordered descending)."""
 import json
@@ -37,7 +37,7 @@ def _check(x_bf16, y_bf16, idx, val, k, min_sim=0.0, self_match=False):
 @pytest.mark.parametrize("two_cta", ["0", "1"])
 @pytest.mark.parametrize("n_from,n_to,d,k", [(6, 3, 300, 3), (300, 700, 768, 10), (129, 257, 64, 1), (1000, 2500, 96, 32), (257, 5000, 200, 5)])
 def test_dense_topk_random(n_from, n_to, d, k, two_cta, monkeypatch):
-    """Both launch shapes: one CTA per 128 from-rows, and CTA pairs (tcgen05 cta_group::2, M = 256, half the to-operand per CTA)."""
+    """Both launch shapes: one CTA per 128 from-rows, and CTA pairs (cluster of 2 sharing each to-tile through TMA multicast)."""
     from polyfuzz_b200 import dense
     monkeypatch.setenv("PFZ_K4_2CTA", two_cta)
     g = torch.Generator().manual_seed(n_from * 7 + d)

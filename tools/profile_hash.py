@@ -1,4 +1,4 @@
-"""Developer tool: K2 hash variant on uniform strings (BASELINE config 5 shape), timing + launches for ncu -k regex:spcos_hash."""
+"""Developer tool: K2 hash variant on uniform strings (BASELINE config 5 shape), timing + launches for a profiler run."""
 import sys, os
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))
 import numpy as np, torch

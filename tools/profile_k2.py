@@ -1,4 +1,4 @@
-"""Developer tool: set up the 100k company-names workload (real fixture when present) and launch K2 a few times (for ncu -k regex:spcos)."""
+"""Developer tool: set up the 100k company-names workload (real fixture when present) and launch K2 a few times (for a profiler run)."""
 import sys, os
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))
 import torch
