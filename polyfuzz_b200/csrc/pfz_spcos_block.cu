@@ -263,8 +263,11 @@ __device__ __forceinline__ unsigned warp_sort_desc_u32(unsigned x, int lane) {
 #ifndef PFZ_B3_ICAP_PER_ROW
 #define PFZ_B3_ICAP_PER_ROW 64
 #endif
+// Register bound: 16 warps per SM, i.e. 128 registers per thread (2 CTAs of 8 rows).  The default 4 096-row tile needs 88 KB of
+// shared memory per 8-row CTA, which stops at 2 CTAs per SM anyway; a 64-register bound (32 warps) only made the kernel spill.
+// On an H100 the 4 096-row tile at this bound takes about a fifth less time than the 2 048-row tile at 64 registers (DESIGN §4.1).
 #ifndef PFZ_B3_MIN_CTAS
-#define PFZ_B3_MIN_CTAS(BF) (32 / (BF))
+#define PFZ_B3_MIN_CTAS(BF) (16 / (BF))
 #endif
 constexpr int B3_ICAP_PER_ROW = PFZ_B3_ICAP_PER_ROW;              // staged work items per unit = 64 x block rows; larger units walk the term table directly
 constexpr int B3_QCAP = 128;                     // candidates a from-row may queue before they are re-scored exactly
@@ -438,7 +441,19 @@ __device__ __forceinline__ void blk3_take_group(const B3Ctx *cx, B3Row *rs, B3St
 
 // one posting chunk applied to the from-rows that hold the term (nf is warp-uniform); idle lanes (pk = 0) add into their dump word.
 // 16-bit mode: pk = {word byte offset | selector << 16, w15}, update = ceil(v16 * w15 / 2^16) in its half-word (IMAD + PRMT);
-// the (row, weight) list is read two entries at a time, the odd tail masked (weight 0 adds 0).
+// 32-bit mode: pk = {tile-local row, w_i}, update = mulhi(v_i, w_i) + 1.  The (row, weight) list is read two entries at a time
+// and an odd tail takes one red of its own: every red adds a real product (69 % of the (block, term) pairs of company names
+// have one row, so a red of weight 0 for the odd tail was 16 % of all reds).
+template <bool P16>
+__device__ __forceinline__ unsigned blk3_update(unsigned v, unsigned wq, unsigned sel) {
+    if (P16) return __byte_perm(v * wq + 0xffffu, 0u, sel);
+    return __umulhi(v, wq) + 1u;
+}
+__device__ __forceinline__ uint2 lds64(unsigned a) {
+    uint2 v;
+    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a));
+    return v;
+}
 template <bool P16>
 __device__ __forceinline__ void blk3_process(int lane, int cnt, unsigned fva, int nf, uint2 pk, unsigned acc_s, unsigned dump_s) {
     unsigned cell, sel = 0u;
@@ -446,30 +461,15 @@ __device__ __forceinline__ void blk3_process(int lane, int cnt, unsigned fva, in
     if (P16) { cell = acc_s + (pk.x & 0xffffu); sel = pk.x >> 16; }
     else cell = acc_s + (pk.x << 2);
     if (lane >= cnt) cell = dump_s;
-    if (P16) {
 #pragma unroll 1
-        for (; nf > 0; nf -= 2, fva += 16u) {
-            uint2 e0, e1;
-            asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(e0.x), "=r"(e0.y) : "r"(fva));
-            asm volatile("ld.shared.v2.u32 {%0, %1}, [%2+8];" : "=r"(e1.x), "=r"(e1.y) : "r"(fva));
-            if (nf == 1) e1.y = 0u;                                 // (the next term's entry, or the sentinel behind the table)
-            red_add_u32(cell + e0.x, __byte_perm(e0.y * wq + 0xffffu, 0u, sel));
-            red_add_u32(cell + e1.x, __byte_perm(e1.y * wq + 0xffffu, 0u, sel));
-        }
-    } else {
-#pragma unroll 1
-        for (; nf >= 2; nf -= 2, fva += 16u) {
-            uint2 e0, e1;
-            asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(e0.x), "=r"(e0.y) : "r"(fva));
-            asm volatile("ld.shared.v2.u32 {%0, %1}, [%2+8];" : "=r"(e1.x), "=r"(e1.y) : "r"(fva));
-            red_add_u32(cell + e0.x, __umulhi(e0.y, wq) + 1u);
-            red_add_u32(cell + e1.x, __umulhi(e1.y, wq) + 1u);
-        }
-        if (nf) {
-            uint2 e0;
-            asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(e0.x), "=r"(e0.y) : "r"(fva));
-            red_add_u32(cell + e0.x, __umulhi(e0.y, wq) + 1u);
-        }
+    for (; nf >= 2; nf -= 2, fva += 16u) {
+        const uint2 e0 = lds64(fva), e1 = lds64(fva + 8u);
+        red_add_u32(cell + e0.x, blk3_update<P16>(e0.y, wq, sel));
+        red_add_u32(cell + e1.x, blk3_update<P16>(e1.y, wq, sel));
+    }
+    if (nf) {
+        const uint2 e0 = lds64(fva);
+        red_add_u32(cell + e0.x, blk3_update<P16>(e0.y, wq, sel));
     }
 }
 
@@ -568,7 +568,7 @@ template <int BF, bool P16>
 __host__ __device__ inline size_t blk3_arena_bytes(int T) {
     return (size_t)BF * (T * (P16 ? 2 : 4) + 128)   // acc: per from-row the tile's cells + 32 dump words (idle lanes)
            + (size_t)BF * B3_ICAP_PER_ROW * 16 // items
-           + (size_t)(BF * 64 + 2) * 8         // fv (+ sentinel)
+           + (size_t)BF * 64 * 8              // fv: (row, weight) table of the block
            + (size_t)BF * sizeof(B3Row)        // per-row filter / top-k state
            + sizeof(B3Ctx) + 64;               // context, counters
 }
@@ -594,8 +594,8 @@ __global__ void __launch_bounds__(BF * 32, PFZ_B3_MIN_CTAS(BF)) spcos_blk3_kerne
     unsigned *acc = reinterpret_cast<unsigned *>(dyn);
     B3Item *items = reinterpret_cast<B3Item *>(dyn + (size_t)BF * RW * 4);
     uint2 *fvtab = reinterpret_cast<uint2 *>(reinterpret_cast<unsigned char *>(items) + (size_t)B3_ICAP * 16);
-    B3Row *rs = reinterpret_cast<B3Row *>(reinterpret_cast<unsigned char *>(fvtab) + (size_t)(FV_CAP + 2) * 8) + w;
-    B3Ctx *cx = reinterpret_cast<B3Ctx *>(reinterpret_cast<unsigned char *>(fvtab) + (size_t)(FV_CAP + 2) * 8 + (size_t)BF * sizeof(B3Row));
+    B3Row *rs = reinterpret_cast<B3Row *>(reinterpret_cast<unsigned char *>(fvtab) + (size_t)FV_CAP * 8) + w;
+    B3Ctx *cx = reinterpret_cast<B3Ctx *>(reinterpret_cast<unsigned char *>(fvtab) + (size_t)FV_CAP * 8 + (size_t)BF * sizeof(B3Row));
     int *misc = reinterpret_cast<int *>(cx + 1);
     int *icnt = misc;                                                   // [2] item counters (tile parity)
     int *bcast = misc + 2;
@@ -669,12 +669,9 @@ __global__ void __launch_bounds__(BF * 32, PFZ_B3_MIN_CTAS(BF)) spcos_blk3_kerne
             int nfv_total = 0;
 #pragma unroll
             for (int q = 0; q < W; ++q) nfv_total += wsum[q];
-            for (int e = tid; e <= nfv_total; e += NT) {
-                uint2 x = make_uint2(0u, 0u);                           // (sentinel behind the table: the masked odd tail reads it)
-                if (e < nfv_total) {
-                    x = P.blk_fv[D.base + e];
-                    if (P16) x.y = max(1u, x.y >> 16);                  // v16 = max(1, floor(v * 2^16))
-                }
+            for (int e = tid; e < nfv_total; e += NT) {
+                uint2 x = P.blk_fv[D.base + e];
+                if (P16) x.y = max(1u, x.y >> 16);                      // v16 = max(1, floor(v * 2^16))
                 fvtab[e] = x;
             }
         }

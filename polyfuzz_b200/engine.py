@@ -425,8 +425,10 @@ class NgramTfidf:
 # to-tile rows per K2 variant: the list kernel wants many small per-warp arenas (occupancy), the dense
 # kernel few large ones (long segments; it pipelines its own loads)
 DEFAULT_TILE = {"list": int(os.environ.get("PFZ_TILE_LIST", "512")), "dense": int(os.environ.get("PFZ_TILE_DENSE", "1024")),
-                "dense32": int(os.environ.get("PFZ_TILE_DENSE32", "1024")), "block": int(os.environ.get("PFZ_TILE_BLOCK", "2048")),
+                "dense32": int(os.environ.get("PFZ_TILE_DENSE32", "1024")), "block": int(os.environ.get("PFZ_TILE_BLOCK", "4096")),
                 "hash": 65536}
+# block kernel: the tile above is for 16-bit accumulators; 32-bit ones take half of it, the same accumulator bytes (a 4 096-row
+# tile of 32-bit accumulators would not fit a 16-row CTA in shared memory)
 BLOCK_TILE_STEP, BLOCK_TILE_MAX = 128, 4096
 BLOCK_ROWS = int(os.environ.get("PFZ_BLOCK_ROWS", "8"))           # from-rows (= warps) per CTA of the block kernel: 4, 8 or 16
 BLOCK_ACC_BITS = int(os.environ.get("PFZ_BLOCK_ACC_BITS", "16"))  # 16: two accumulators per word (unit 2^-15); 32: one per word (2^-26)
@@ -440,6 +442,8 @@ class SparseIndex:
         self.variant = variant
         if tile is None:
             tile = DEFAULT_TILE[variant]
+            if variant == "block" and BLOCK_ACC_BITS != 16:
+                tile //= 2
         tile = max(64, min(int(tile), ((max(n, 1) + 63) // 64) * 64))
         self.acc_bits = 32
         if variant == "block":                                # the block kernel scans its accumulators 128 words per warp step
