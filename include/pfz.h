@@ -35,6 +35,8 @@ extern "C" {
 #define PFZ_METRIC_INDEL     1     /* |a|+|b|-2*LCS                                                */
 #define PFZ_METRIC_NORM_LEV  2     /* 1 - lev/max(|a|,|b|)                                         */
 #define PFZ_METRIC_RATIO     3     /* rapidfuzz fuzz.ratio = (1 - indel/(|a|+|b|))*100             */
+#define PFZ_METRIC_JARO      4     /* jellyfish jaro_similarity(from, to), in [0, 1]                */
+#define PFZ_METRIC_JARO_WINKLER 5  /* jellyfish jaro_winkler_similarity(from, to), long_tolerance=False */
 
 int         pfz_abi_version(void);
 const char *pfz_last_error(void);
@@ -224,11 +226,15 @@ int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32
 
 /* scores the from-strings listed in from_ids (all of one word class: n_words = 0 -> length <= 32 (one
  * 32-bit word), 1/2/4/8/16 -> length <= 64*n_words) against every to-string.
- *   metric: PFZ_METRIC_*; for NORM_LEV / RATIO a candidate needs score >= score_cutoff
+ *   metric: PFZ_METRIC_*; for NORM_LEV / RATIO / JARO / JARO_WINKLER a candidate needs score >= score_cutoff
  *   exclude_self: skip to-row == from-row + self_shift
- *   part_*: [n_splits][n_from] partial bests (merge with pfz_lev_merge); ties -> lowest to-index
- *   matrix (may be NULL): int32 [n_from][matrix_ld] full distance matrix (Levenshtein or Indel)
- *   counter: int32[n_splits], zeroed by the callee                                                   */
+ *   part_*: [n_splits][n_from] partial bests (merge with pfz_lev_merge); ties -> lowest to-index;
+ *           part_dist holds the distance, or for JARO / JARO_WINKLER the number of matching characters
+ *   matrix (may be NULL): int32 [n_from][matrix_ld] full distance matrix (Levenshtein or Indel); must be
+ *           NULL for JARO / JARO_WINKLER
+ *   counter: int32[n_splits], zeroed by the callee
+ * JARO / JARO_WINKLER: jellyfish's definition on code points, from-string first (the reference calls
+ * scorer(from_string, to_string), polyfuzz/models/_distance.py:98); DESIGN.md 4.5 gives the recurrence.  */
 int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
                     int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
                     const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,

@@ -1,5 +1,5 @@
-// pfz_lev.cu -- K3: all-pairs edit distance (bit-parallel Myers/Hyyro Levenshtein and Hyyro LCS/Indel)
-// over the |from| x |to| grid with a fused per-row arg-best.
+// pfz_lev.cu -- K3: all-pairs edit distance (bit-parallel Myers/Hyyro Levenshtein and Hyyro LCS/Indel) and
+// Jaro / Jaro-Winkler similarity over the |from| x |to| grid with a fused per-row arg-best.
 //
 // Replaces rapidfuzz's scorer loop as the reference calls it:
 //     polyfuzz/models/_rapidfuzz.py:99-113  process.extractOne(q, to_list, score_cutoff, scorer=fuzz.ratio)
@@ -222,6 +222,147 @@ __global__ void __launch_bounds__(WARPS * 32) lev_kernel(const LevParams P) {
     }
 }
 
+// Jaro / Jaro-Winkler (jellyfish's definition, s1 = pattern = from-string, s2 = text = to-string).  The text-driven greedy:
+// text symbol j takes the LOWEST unflagged pattern position i with |i - j| <= R and P[i] == T[j]; it flags the same pairs
+// as the definition's pattern-driven loop (rapidfuzz's bit-parallel Jaro).  Pflag holds the flagged pattern bits; the
+// lane records its matched text symbols in order in shared memory (<= min(m, n) bytes, column `lane` of the warp's
+// store), so the transposition count pairs the k-th stored symbol with the k-th lowest Pflag bit: a mismatch iff
+// bit i of Peq[stored k] is clear.  Scores are the definition's float64 expression, rounded step by step.
+template <typename W>
+__device__ __forceinline__ W window_bits(int lo, int hi) {      // bits lo..hi of one block (block-relative, may lie outside)
+    constexpr int B = WordOps<W>::BITS;
+    if (hi < 0 || lo >= B) return 0;
+    const W up = hi >= B - 1 ? ~(W)0 : (((W)1 << (hi + 1)) - 1);
+    const W dn = lo <= 0 ? ~(W)0 : ~(((W)1 << lo) - 1);
+    return up & dn;
+}
+
+template <typename W> __device__ __forceinline__ int low_bit(W x);
+template <> __device__ __forceinline__ int low_bit<uint32_t>(uint32_t x) { return __ffs(x) - 1; }
+template <> __device__ __forceinline__ int low_bit<uint64_t>(uint64_t x) { return __ffsll(x) - 1; }
+
+template <typename W, int NW, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
+    constexpr int B = WordOps<W>::BITS;
+    constexpr int STORE = B * NW;                                           // max matches per lane
+    extern __shared__ __align__(16) unsigned char dyn[];
+    const int lane = lane_id();
+    const int w = threadIdx.x >> 5;
+    W *peq = reinterpret_cast<W *>(dyn) + (size_t)w * 256 * NW;              // peq[sym * NW + block]
+    uint8_t *store = dyn + (size_t)WARPS * 256 * NW * sizeof(W) + (size_t)w * STORE * 32 + lane;    // store[k * 32]
+    const bool winkler = P.metric == PFZ_METRIC_JARO_WINKLER;
+    const int split = blockIdx.y;
+    const int n_grp = (P.n_to + 31) >> 5;
+    const int per = (n_grp + P.n_splits - 1) / P.n_splits;
+    const int g_lo = split * per, g_hi = min(n_grp, g_lo + per);
+    int32_t *counter = P.counter + split;
+
+    for (;;) {
+        int q = 0;
+        if (lane == 0) q = atomicAdd(counter, 1);
+        q = __shfl_sync(FULL, q, 0);
+        if (q >= P.n_ids) break;
+        const int i = P.from_ids[q];
+        const int64_t fb = P.from_off[i];
+        const int m = (int)(P.from_off[i + 1] - fb);
+        for (int e = lane; e < 256 * NW; e += 32) peq[e] = 0;
+        __syncwarp();
+        for (int p = lane; p < m; p += 32) {
+            const uint32_t c = P.from_blob[fb + p];
+            const int s = c < 0x110000u ? P.sym_table[c] : 0;
+            if (s) {
+                if (sizeof(W) == 8) atomicOr(reinterpret_cast<unsigned long long *>(&peq[s * NW + p / B]), 1ull << (p % B));
+                else atomicOr(reinterpret_cast<unsigned *>(&peq[s * NW + p / B]), 1u << (p % B));
+            }
+        }
+        __syncwarp();
+        const int last_blk = m > 0 ? (m - 1) / B : 0;                          // blocks above it hold no pattern bits
+
+        double best_s = 0.0; int best_j = -1, best_d = -1;
+        for (int g = g_lo; g < g_hi; ++g) {
+            const int p = g * 32 + lane;
+            const bool have = p < P.n_to;
+            const int n = have ? P.slen[p] : 0;
+            const int orig = have ? P.sorig[p] : -1;
+            const int R = max(0, max(m, n) / 2 - 1);
+            const int jend = m > 0 ? min(n, m + R) : 0;                  // text positions >= m + R have an empty window
+            int jmax = jend;
+#pragma unroll
+            for (int d = 16; d; d >>= 1) jmax = max(jmax, __shfl_xor_sync(FULL, jmax, d));
+            const uint32_t *src = P.packed + P.grp_word_off[g] + lane;
+            const uint32_t first = n > 0 ? src[0] : 0u;
+            W F[NW], win[NW];                                                // win: pattern bits j-R .. j+R
+#pragma unroll
+            for (int b = 0; b < NW; ++b) { F[b] = 0; win[b] = window_bits<W>(-b * B, R - b * B); }
+            int k = 0;
+            uint32_t nextw = first;
+            for (int j0 = 0; j0 < jmax; j0 += 4) {
+                const uint32_t word = nextw;
+                if (j0 + 4 < jmax) nextw = src[(size_t)((j0 >> 2) + 1) * 32];
+#pragma unroll
+                for (int bb = 0; bb < 4; ++bb) {
+                    const int j = j0 + bb;
+                    const int s = (word >> (8 * bb)) & 0xff;
+                    if (j < jend && s) {
+                        bool found = false;
+#pragma unroll
+                        for (int b = 0; b < NW; ++b) {
+                            if (b <= last_blk) {
+                                const W x = peq[s * NW + b] & ~F[b] & win[b];
+                                if (!found && x) { F[b] |= x & (~x + 1); found = true; }
+                            }
+                        }
+                        if (found) { store[(size_t)k * 32] = (uint8_t)s; ++k; }
+                    }
+                    // slide the window one position: shift left across blocks; bit 0 stays set while j + 1 <= R
+#pragma unroll
+                    for (int b = NW - 1; b >= 0; --b) {
+                        if (b <= last_blk) win[b] = (win[b] << 1) | (b > 0 ? win[b > 0 ? b - 1 : 0] >> (B - 1) : (W)(j + 1 <= R));
+                    }
+                }
+            }
+            int trans = 0, kk = 0;
+#pragma unroll
+            for (int b = 0; b < NW; ++b) {
+                W f = F[b];
+                while (f) {
+                    const int bit = low_bit<W>(f);
+                    f &= f - 1;
+                    const int s = store[(size_t)kk * 32];
+                    ++kk;
+                    trans += !((peq[s * NW + b] >> bit) & 1);
+                }
+            }
+            double sc = 0.0;
+            if (k > 0) {
+                const double dm = (double)k;
+                sc = __ddiv_rn(__dadd_rn(__dadd_rn(__ddiv_rn(dm, (double)m), __ddiv_rn(dm, (double)n)), __ddiv_rn(__dsub_rn(dm, (double)(trans / 2)), dm)), 3.0);
+                if (winkler && sc > 0.7) {
+                    const int cap = min(min(m, n), 4);
+                    int pre = 0;
+                    while (pre < cap && ((peq[((first >> (8 * pre)) & 0xff) * NW] >> pre) & 1)) ++pre;
+                    if (pre > 0) sc = __dadd_rn(sc, __dmul_rn(__dmul_rn((double)pre, 0.1), __dsub_rn(1.0, sc)));
+                }
+            }
+            if (have) {
+                bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) && sc >= P.cutoff;
+                if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = k; }
+            }
+        }
+#pragma unroll
+        for (int d = 16; d; d >>= 1) {
+            const double os = shfl_d(best_s, lane ^ d);
+            const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
+            if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
+        }
+        if (lane == 0) {
+            const size_t o = (size_t)split * P.n_from + i;
+            P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
+        }
+        __syncwarp();
+    }
+}
+
 __global__ void lev_merge_kernel(const int32_t *__restrict__ part_idx, const double *__restrict__ part_score, const int32_t *__restrict__ part_dist,
                                  int n_splits, int n_from, int32_t *__restrict__ best_idx, double *__restrict__ best_score,
                                  int32_t *__restrict__ best_dist) {
@@ -256,6 +397,27 @@ static int launch_lev(const LevParams &P, int sms, cudaStream_t st) {
     return 0;
 }
 
+// Shared memory per warp: Peq (256 x NW words) plus the match store (32 lanes x B*NW bytes), the same size again.
+// Up to 64 KB per CTA: 4 warps up to 256 code points, 2 at 512, 1 at 1 024.
+template <typename W, int NW>
+static int launch_jaro(const LevParams &P, int sms, cudaStream_t st) {
+    constexpr size_t PER_WARP = 2 * 256 * NW * sizeof(W);
+    constexpr int WARPS = PER_WARP * 4 <= 65536 ? 4 : PER_WARP * 2 <= 65536 ? 2 : 1;
+    const size_t smem = (size_t)WARPS * PER_WARP;
+    auto kernel = jaro_kernel<W, NW, WARPS>;
+    PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int occ = 0;
+    PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
+    if (occ < 1) occ = 1;
+    int gx = sms * occ;
+    const int need = (P.n_ids + WARPS - 1) / WARPS;
+    if (gx > need) gx = need;
+    if (gx < 1) gx = 1;
+    kernel<<<dim3(gx, P.n_splits), WARPS * 32, smem, st>>>(P);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
 }  // namespace pfz
 
 using namespace pfz;
@@ -277,10 +439,12 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
                     const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
                     int32_t n_splits, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
                     int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_RATIO, "pfz_lev_argbest: unknown metric %d", metric);
+    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_JARO_WINKLER, "pfz_lev_argbest: unknown metric %d", metric);
     PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
                 "pfz_lev_argbest: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
     PFZ_REQUIRE(n_splits >= 1, "pfz_lev_argbest: n_splits < 1");
+    const bool jaro = metric == PFZ_METRIC_JARO || metric == PFZ_METRIC_JARO_WINKLER;
+    PFZ_REQUIRE(!(jaro && matrix), "pfz_lev_argbest: the distance matrix is not available for the Jaro metrics (matrix must be NULL)");
     if (n_ids <= 0 || n_to < 0) return 0;
     cudaStream_t st = as_stream(stream);
     int dev = 0, sms = 0;
@@ -289,6 +453,16 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
     PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
     LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
                 exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter};
+    if (jaro) {
+        switch (n_words) {
+            case 0: return launch_jaro<uint32_t, 1>(P, sms, st);
+            case 1: return launch_jaro<uint64_t, 1>(P, sms, st);
+            case 2: return launch_jaro<uint64_t, 2>(P, sms, st);
+            case 4: return launch_jaro<uint64_t, 4>(P, sms, st);
+            case 8: return launch_jaro<uint64_t, 8>(P, sms, st);
+            default: return launch_jaro<uint64_t, 16>(P, sms, st);
+        }
+    }
     const bool lcs = (metric == PFZ_METRIC_INDEL || metric == PFZ_METRIC_RATIO);
 #define PFZ_LEV_CASE(NWv, Wt)                                                            \
     return lcs ? launch_lev<Wt, NWv, true>(P, sms, st) : launch_lev<Wt, NWv, false>(P, sms, st)

@@ -5,6 +5,11 @@ polyfuzz/models/_distance.py:89-102) and rapidfuzz's published definitions:
     "ratio"     fuzz.ratio           = (1 - indel/(|a|+|b|)) * 100            in [0, 100]
     "norm_lev"  Levenshtein.normalized_similarity = 1 - lev/max(|a|,|b|)       in [0, 1]
     "lev", "indel"  raw distances (best = smallest)
+    "jaro"          jellyfish.jaro_similarity(from, to)                          in [0, 1]
+    "jaro_winkler"  jellyfish.jaro_winkler_similarity(from, to), long_tolerance=False   in [0, 1]
+The Jaro metrics are computed on code points, from-string first (the reference calls scorer(from_string, to_string),
+polyfuzz/models/_distance.py:98); their best_dist is the number of matching characters, and they have no distance
+matrix (want_matrix=True raises ValueError).
 Best match of a from-string = first to-string (lowest index) with the maximal score >= score_cutoff.
 
 Two levels: `EditQueries` / `EditTargets` stage a from-list / to-list in HBM once (host packing, length sort,
@@ -18,7 +23,8 @@ from . import _lib
 from .engine import _dev, _p, _stream, _to_dev
 from .strings import pack_strings
 
-METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3}
+METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3, "jaro": 4, "jaro_winkler": 5}
+JARO_METRICS = ("jaro", "jaro_winkler")
 N_CODE_POINTS = 0x110000
 MAX_LEN = 1024
 
@@ -131,6 +137,8 @@ def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=Fal
                         n_splits=None, to_index_base=0):
     """Kernels only.  Returns (best_idx int32[n_from] (-1 = none; + to_index_base otherwise), best_score float64[n_from],
     best_dist int32[n_from] [, matrix int32[n_from, n_to]]) as device tensors."""
+    if want_matrix and metric in JARO_METRICS:
+        raise ValueError(f"want_matrix=True: the {metric!r} metric has no integer distance matrix")
     dev = _dev()
     n_from, n_to = Q.n, T.n
     best_idx = torch.full((max(n_from, 1),), -1, dtype=torch.int32, device=dev)

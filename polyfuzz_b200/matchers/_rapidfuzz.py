@@ -9,7 +9,10 @@ published known answers):
     "partial_token_ratio"                                         -> csrc/pfz_fuzz.cu (K3b)
   * "ratio" (fuzz.ratio, the reference's default for EditDistance, _distance.py:32) and "levenshtein"
     (Levenshtein.normalized_similarity)                                  -> csrc/pfz_lev.cu (K3)
-A scorer may be given by name or as the rapidfuzz callable of that __name__.  Arbitrary Python callables cannot be
+  * EditDistance only: "jaro_similarity" / "jaro" and "jaro_winkler_similarity" / "jaro_winkler" (jellyfish's
+    definitions with long_tolerance=False, the custom scorer of the reference's tutorial; raw 0..1 scores)
+                                                                         -> csrc/pfz_lev.cu (K3, Jaro mode)
+A scorer may be given by name or as the rapidfuzz / jellyfish callable of that __name__.  Arbitrary Python callables cannot be
 compiled to the device and raise NotImplementedError -- there is no CPU fallback.
 Deviations from the reference, both documented reference bugs (SURVEY.md 8a): a self-match excludes
 index i only (the reference mutates the shared to_list, _rapidfuzz.py:103-104), and the matcher can be
@@ -26,10 +29,12 @@ from ..distributed import get_comm, shard_bounds
 _NAMES = {"ratio": "ratio", "levenshtein": "norm_lev", "norm_lev": "norm_lev", "normalized_similarity": "norm_lev",
           "normalized_levenshtein": "norm_lev"}
 _FUZZ = {k.lower(): k for k in fuzzy.SCORER if k != "ratio"}
+# jellyfish's function names (and short forms); 0..1 scores, so only EditDistance takes them
+_JARO = {"jaro": "jaro", "jaro_similarity": "jaro", "jaro_winkler": "jaro_winkler", "jaro_winkler_similarity": "jaro_winkler"}
 
 
-def _resolve_scorer(scorer, default) -> str:
-    """-> "ratio" | "norm_lev" (K3) or one of fuzzy.SCORER (K3b)."""
+def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
+    """-> "ratio" | "norm_lev" | "jaro" | "jaro_winkler" (K3) or one of fuzzy.SCORER (K3b)."""
     if scorer is None:
         scorer = default
     key = scorer.lower() if isinstance(scorer, str) else getattr(scorer, "__name__", "").lower()
@@ -37,8 +42,11 @@ def _resolve_scorer(scorer, default) -> str:
         return _NAMES[key]
     if key in _FUZZ:
         return _FUZZ[key]
+    if allow_jaro and key in _JARO:
+        return _JARO[key]
     raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: 'ratio', 'levenshtein', "
-                              f"{sorted(_FUZZ.values())}); polyfuzz_b200 has no CPU fallback")
+                              f"{sorted(_FUZZ.values())}" + (", 'jaro_similarity', 'jaro_winkler_similarity'" if allow_jaro else "")
+                              + "); polyfuzz_b200 has no CPU fallback")
 
 
 def _argbest(from_list, targets, metric, cutoff, self_match, distributed):
@@ -99,8 +107,8 @@ class RapidFuzz(BaseMatcher):
 
 class EditDistance(BaseMatcher):
     """Edit-distance matcher with the reference's EditDistance surface (n_jobs, scorer, model_id, normalize):
-    Similarity is the scorer's raw value (fuzz.ratio: 0..100) of the best to-string, min-max normalised
-    over the column when `normalize` (polyfuzz/models/_distance.py:83-86)."""
+    Similarity is the scorer's raw value (fuzz.ratio: 0..100, Jaro / Jaro-Winkler: 0..1) of the best to-string,
+    min-max normalised over the column when `normalize` (polyfuzz/models/_distance.py:83-86)."""
 
     def __init__(self, n_jobs: int = 1, scorer: Union[str, Callable] = "ratio", model_id: str = None, normalize: bool = True,
                  distributed: bool = False):
@@ -108,7 +116,7 @@ class EditDistance(BaseMatcher):
         self.type = "EditDistance"
         self.distributed = distributed
         self.scorer = scorer
-        self._metric = _resolve_scorer(scorer, "ratio")
+        self._metric = _resolve_scorer(scorer, "ratio", allow_jaro=True)
         self.normalize = normalize
         self.equal_lists = False
         self.n_jobs = n_jobs
