@@ -279,6 +279,45 @@ int pfz_dense_cos_topk(const void *x_bf16, const void *y_bf16, int32_t n_from, i
                        double min_similarity, int32_t self_match, int64_t from_index_base, int64_t to_index_base,
                        int32_t n_splits, int32_t *top_idx, double *top_val, void *stream);
 
+/* K4 exact mode: the canonical fp64 cosine top-k (DESIGN.md 2 and 4.6), bit for bit, from an fp16 tensor-core filter pass,
+ * fp64 re-scoring of its candidates with a per-row certificate, and a brute-force pass for the rows not certified.
+ * Canonical dot(a, b): lane l = dimension mod 32 sums a[32t+l]*b[32t+l] over ascending t (products rounded, then added, no
+ * FMA, from +0), then p[l] += p[l xor o] for o = 16, 8, 4, 2, 1.  Normalisation x~ = x / sqrt(dot(x, x)) (a row with
+ * dot(x, x) == 0 stays as it is).  score = dot(x~, y~); candidate iff score > min_similarity (strict) and not the diagonal
+ * (self_match); key (score desc, index asc); empty slots (-1, 0.0).
+ *
+ * prep: rows (float32 or float64, pitch ld) -> out_f64 = x~ and out_f16 = fp16(x~), both [n_rows][d_pad] zero-padded,
+ *   d_pad % 8 == 0; norm16[i] >= ||fp16(x~_i)|| and err16[i] >= ||x~_i - fp16(x~_i)|| (float64[n_rows], upward-rounded);
+ *   maxima (may be NULL): float64[2] = {max norm16, max err16}, zeroed by the callee.                                     */
+int pfz_rows_prep_exact(const void *x, int32_t is_f64, int64_t ld, int32_t n_rows, int32_t d, int32_t d_pad,
+                        double *out_f64, void *out_f16, double *norm16, double *err16, double *maxima, void *stream);
+
+/* filter pass: as pfz_dense_cos_topk on fp16 operands (wgmma .f16), except that the candidates are the fp32 scores > t_f,
+ * t_f = the largest float <= min_similarity - M_max(d), M_max(d) the a-priori bound on |fp32 filter score - canonical
+ * score| of DESIGN.md 4.6.  Every to-row whose canonical score exceeds min_similarity scores above t_f here.           */
+int pfz_dense_cos_topk_f16(const void *x_f16, const void *y_f16, int32_t n_from, int32_t n_to, int32_t d, int32_t k,
+                           double min_similarity, int32_t self_match, int64_t from_index_base, int64_t to_index_base,
+                           int32_t n_splits, int32_t *top_idx, double *top_val, void *stream);
+
+/* re-score + certify: cand_idx / cand_val [n_from][k_cand] = the merged filter lists (global indices) of
+ * pfz_dense_cos_topk_f16 with the same min_similarity; x_* from pfz_rows_prep_exact of the from-rows, y_maxima its maxima
+ * of the to-rows.  k <= k_cand <= 32.  Writes the canonical top-k of every row to top_idx / top_val [n_from][k]; rows whose
+ * result cannot be certified exact are listed in fb_rows (int32[n_from]) with their number in *fb_count (zeroed by the
+ * callee); pfz_dense_exact_fallback overwrites them.                                                                     */
+int pfz_dense_exact_rescore(const double *x_f64, const double *y_f64, int32_t n_from, int32_t n_to, int32_t d_pad, int32_t k,
+                            int32_t k_cand, const int32_t *cand_idx, const double *cand_val, const double *x_norm16,
+                            const double *x_err16, const double *y_maxima, double min_similarity, int32_t self_match,
+                            int64_t from_index_base, int64_t to_index_base, int32_t *top_idx, double *top_val,
+                            int32_t *fb_rows, int32_t *fb_count, void *stream);
+
+/* fallback: canonical top-k over every to-row for the *fb_count rows in fb_rows (the count is read on the device).
+ * ws: >= pfz_dense_exact_fallback_ws_bytes(n_from, n_to, k) bytes.                                                       */
+int64_t pfz_dense_exact_fallback_ws_bytes(int32_t n_from, int32_t n_to, int32_t k);
+int pfz_dense_exact_fallback(const double *x_f64, const double *y_f64, int32_t n_from, int32_t n_to, int32_t d_pad, int32_t k,
+                             double min_similarity, int32_t self_match, int64_t from_index_base, int64_t to_index_base,
+                             const int32_t *fb_rows, const int32_t *fb_count, int32_t *top_idx, double *top_val, void *ws,
+                             void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * K5  frame tail: top-k arrays -> the columns of the result frame (csrc/pfz_assemble.cu).
  * Replaces: polyfuzz/models/_utils.py:104-125 (the per-rank `[to_list[idx] ...]` gathers, the 3-decimal rounding of :102/:143

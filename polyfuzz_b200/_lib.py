@@ -46,8 +46,15 @@ _PROTOS = {
     "pfz_frame_tail_copy": [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_rows_to_bf16": [c_vp, c_i32, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp],
     "pfz_dense_cos_topk": [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp],
+    "pfz_rows_prep_exact": [c_vp, c_i32, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    "pfz_dense_cos_topk_f16": [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp],
+    "pfz_dense_exact_rescore": [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_f64, c_i32, c_i64, c_i64,
+                                c_vp, c_vp, c_vp, c_vp, c_vp],
+    "pfz_dense_exact_fallback_ws_bytes": [c_i32, c_i32, c_i32],
+    "pfz_dense_exact_fallback": [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
 }
-_RESTYPES = {"pfz_last_error": ctypes.c_char_p, "pfz_scan_ws_bytes": c_i64, "pfz_launch_count": c_i64, "pfz_spcos_block_ws_bytes": c_i64}
+_RESTYPES = {"pfz_last_error": ctypes.c_char_p, "pfz_scan_ws_bytes": c_i64, "pfz_launch_count": c_i64, "pfz_spcos_block_ws_bytes": c_i64,
+             "pfz_dense_exact_fallback_ws_bytes": c_i64}
 
 
 def exported_names():

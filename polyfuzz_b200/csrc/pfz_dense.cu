@@ -16,8 +16,15 @@
 // Cluster variant (MCAST): a pair of CTAs (cluster of 2) works on two adjacent 128-row blocks against the same
 // to-tiles.  Each CTA loads one half of the Y tile and multicasts it into both CTAs' shared memory, which halves
 // the to-operand L2 -> SM traffic per CTA; a stage is refilled only once the consumers of both CTAs released it.
+//
+// Exact mode (Embeddings(precision="fp64"), DESIGN.md 4.6): rows_prep_exact_kernel stages canonical fp64 rows and their fp16
+// rounding with error bounds, the same GEMM kernel on fp16 operands filters k' candidates per row below a margin, and
+// exact_rescore_kernel scores them in fp64 and certifies the row; exact_fallback_kernel scores the rows it could not certify
+// against every to-row.
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <math.h>
 #include <stdlib.h>
 #include "pfz_common.cuh"
 
@@ -73,25 +80,30 @@ template <int R> __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
-// D (+)= A[smem] * B[smem]^T, bf16 inputs, fp32 accumulate; scale_d == 0 overwrites D
+// D (+)= A[smem] * B[smem]^T, bf16 (or fp16) inputs, fp32 accumulate; scale_d == 0 overwrites D
+#define PFZ_WGMMA_M64N128K16(AB)                                                                                          \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                       \
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32." AB "." AB " {"                                               \
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                    \
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                          \
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                          \
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"                            \
+                 "}, %64, %65, p, 1, 1, 0, 0;\n\t}"                                                                         \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),           \
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),     \
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),   \
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),   \
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),   \
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),   \
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),   \
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])    \
+                 : "l"(adesc), "l"(bdesc), "r"(scale_d))
+template <bool F16>
 __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
-                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-                 "}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-                 : "l"(adesc), "l"(bdesc), "r"(scale_d));
+    if constexpr (F16) PFZ_WGMMA_M64N128K16("f16");
+    else PFZ_WGMMA_M64N128K16("bf16");
 }
+#undef PFZ_WGMMA_M64N128K16
 
 struct DenseParams {
     int n_from, n_to, d; int k; float min_sim; int self_match; long long from_base, to_base;
@@ -112,7 +124,8 @@ __device__ __forceinline__ void topk_insert(float (&tv)[KMAX], int (&ti)[KMAX], 
     }
 }
 
-template <int KMAX, bool MCAST>
+// F16: operands are fp16 instead of bf16 (the filter pass of the exact mode); nothing else differs
+template <int KMAX, bool MCAST, bool F16>
 __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const __grid_constant__ CUtensorMap map_x,
                                                                           const __grid_constant__ CUtensorMap map_y, const DenseParams P) {
     constexpr int S = DSTAGES, G = MCAST ? 2 : 1;
@@ -196,7 +209,7 @@ __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const 
 #pragma unroll
                     for (int kk = 0; kk < DK / WG_K; ++kk)
                         // advance 16 elements = 32 bytes along K inside the 128-byte swizzled row: +2 in the address field
-                        wgmma_m64n128(acc, ad + (uint64_t)(kk * 2), bd + (uint64_t)(kk * 2), (kb | kk) ? 1 : 0);
+                        wgmma_m64n128<F16>(acc, ad + (uint64_t)(kk * 2), bd + (uint64_t)(kk * 2), (kb | kk) ? 1 : 0);
                     wgmma_commit();
                     wgmma_wait<1>();                                     // the previous stage's MMAs have retired
                     if (prev >= 0) release(prev);
@@ -283,29 +296,265 @@ __global__ void __launch_bounds__(256) rows_normalize_bf16_kernel(const T *__res
     }
 }
 
+// ---- exact mode: canonical fp64 scores, certified against an fp16 tensor-core filter pass (DESIGN.md 4.6) ----------------
+//
+// canonical dot(a, b): lane l sums a[32 t + l] * b[32 t + l] over ascending t (product rounded, then added; no FMA; from +0),
+// then p[l] += p[l ^ o] for o = 16, 8, 4, 2, 1.  Every lane ends with the same value.  Zero padding up to d_pad adds +0 and
+// changes nothing.
+
+__device__ __forceinline__ double warp_sum_rn(double p) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) p = __dadd_rn(p, __shfl_xor_sync(FULL, p, o));
+    return p;
+}
+__device__ __forceinline__ double warp_sum_ru(double p) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) p = __dadd_ru(p, __shfl_xor_sync(FULL, p, o));
+    return p;
+}
+
+// NC canonical dots of one row a against rows b[0..NC-1], interleaved for memory-level parallelism
+template <int NC>
+__device__ __forceinline__ void warp_dot_canon(const double *__restrict__ a, const double *const (&b)[NC], int d_pad, int lane, double (&out)[NC]) {
+    double p[NC];
+#pragma unroll
+    for (int u = 0; u < NC; ++u) p[u] = 0.0;
+    for (int c = lane; c < d_pad; c += 32) {
+        const double av = a[c];
+#pragma unroll
+        for (int u = 0; u < NC; ++u) p[u] = __dadd_rn(p[u], __dmul_rn(av, b[u][c]));
+    }
+#pragma unroll
+    for (int u = 0; u < NC; ++u) out[u] = warp_sum_rn(p[u]);
+}
+
+// rows -> canonical l2-normalised fp64 rows x~ and their fp16 rounding x^ ([n_rows][d_pad], zero padded), with upper bounds
+// of ||x^|| and ||x~ - x^|| per row and (maxima, may be NULL) of both over all rows.  One warp per row.
+template <typename T>
+__global__ void __launch_bounds__(256) rows_prep_exact_kernel(const T *__restrict__ x, int64_t ld, int n_rows, int d, int d_pad,
+                                                              double *__restrict__ out64, __half *__restrict__ out16, double *__restrict__ norm16,
+                                                              double *__restrict__ err16, unsigned long long *__restrict__ maxima) {
+    const int lane = threadIdx.x & 31;
+    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+    for (int r = gw; r < n_rows; r += nw) {
+        const T *row = x + (int64_t)r * ld;
+        double p = 0.0;
+        for (int c = lane; c < d; c += 32) { const double v = (double)row[c]; p = __dadd_rn(p, __dmul_rn(v, v)); }
+        p = warp_sum_rn(p);
+        const double nrm = __dsqrt_rn(p);
+        double sn = 0.0, se = 0.0;
+        for (int c = lane; c < d_pad; c += 32) {
+            double v = c < d ? (double)row[c] : 0.0;
+            if (p > 0.0) v = __ddiv_rn(v, nrm);                        // a zero row stays as it is
+            const __half h = __double2half(v);
+            const double hv = (double)__half2float(h);
+            const double e = __dsub_rn(v, hv);                         // exact: |e| <= half an fp16 ulp of v
+            out64[(int64_t)r * d_pad + c] = v;
+            out16[(int64_t)r * d_pad + c] = h;
+            sn = __dadd_ru(sn, __dmul_ru(hv, hv));
+            se = __dadd_ru(se, __dmul_ru(e, e));
+        }
+        const double nx = __dsqrt_ru(warp_sum_ru(sn)), ex = __dsqrt_ru(warp_sum_ru(se));
+        if (lane == 0) {
+            norm16[r] = nx; err16[r] = ex;
+            if (maxima) {                                              // non-negative doubles order as their bit patterns
+                atomicMax(&maxima[0], (unsigned long long)__double_as_longlong(nx));
+                atomicMax(&maxima[1], (unsigned long long)__double_as_longlong(ex));
+            }
+        }
+    }
+}
+
+// A-priori bound M_max >= every row's M_i (see exact_rescore_kernel) for rows of width d_pad: |x~| <= r, each fp16 rounding
+// error <= 2^-11 |x~_c| (normal range) + 2^-25 (subnormal range), fp32 accumulation error <= gamma * ||x^|| ||y^||.
+static double exact_gamma(int d_pad) { return d_pad * 0x1p-22; }
+static double exact_margin_max(int d_pad) {
+    const double r = 1.0 + d_pad * 0x1p-50;
+    const double e = 0x1p-11 * r + 0x1p-25 * sqrt((double)d_pad);
+    const double n = r + e;
+    const double m = 2.0 * e * n + e * e + exact_gamma(d_pad) * n * n + 2.0 * d_pad * 0x1p-53 * (n + e) * (n + e);
+    return m * (1.0 + 0x1p-20);
+}
+
+struct ExactParams {
+    const double *x, *y; int n_from, n_to, d_pad, k, kc; double thr, gamma, m_max; int self_match; long long from_base, to_base;
+    const int32_t *cand_idx; const double *cand_val; const double *x_norm, *x_err; const double *y_max;
+    int32_t *top_idx; double *top_val; int32_t *fb_rows; int32_t *fb_count;
+};
+
+// One warp per from-row: canonical scores of the row's <= kc filter candidates (lane c holds candidate c), the exact top-k of
+// the eligible ones, and the certificate that no other to-row belongs in it.  With s_kc the kc-th filter score and
+//   M_i = e_x N_y + n_x E_y + e_x E_y + gamma n_x N_y + 2 d_pad 2^-53 (n_x + e_x)(N_y + E_y)   (rounded up)
+// every non-candidate's canonical score is <= B = s_kc + M_i.  Certified iff: the filter returned fewer than kc candidates
+// (then every non-candidate scored <= t_f <= thr - M_max in fp32, and M_i <= M_max), or B <= thr, or the exact k-th score > B.
+// Other rows are appended to fb_rows.
+__global__ void __launch_bounds__(256) exact_rescore_kernel(const ExactParams P) {
+    const int lane = threadIdx.x & 31;
+    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+    const double Ny = P.y_max[0], Ey = P.y_max[1];
+    constexpr int NC = 4;
+    for (int i = gw; i < P.n_from; i += nw) {
+        const double *xr = P.x + (int64_t)i * P.d_pad;
+        const int my_j = lane < P.kc ? P.cand_idx[(int64_t)i * P.kc + lane] : -1;       // global to-index; the valid ones are a prefix
+        const int nc = __popc(__ballot_sync(FULL, my_j >= 0));
+        double my_s = 0.0;
+        for (int c0 = 0; c0 < nc; c0 += NC) {
+            const double *yr[NC]; double s[NC];
+#pragma unroll
+            for (int u = 0; u < NC; ++u) {
+                const int j = __shfl_sync(FULL, my_j, min(c0 + u, nc - 1));
+                yr[u] = P.y + ((int64_t)j - P.to_base) * P.d_pad;
+            }
+            warp_dot_canon<NC>(xr, yr, P.d_pad, lane, s);
+#pragma unroll
+            for (int u = 0; u < NC; ++u) if (lane == c0 + u) my_s = s[u];
+        }
+        const long long self_j = P.from_base + i;
+        const bool elig = my_j >= 0 && my_s > P.thr && !(P.self_match && (long long)my_j == self_j);
+        const unsigned emask = __ballot_sync(FULL, elig);
+        const int n_el = __popc(emask);
+        int rank = 0;
+#pragma unroll 4
+        for (int z = 0; z < 32; ++z) {
+            const double os = __shfl_sync(FULL, my_s, z); const int oj = __shfl_sync(FULL, my_j, z);
+            if (((emask >> z) & 1u) && (os > my_s || (os == my_s && oj < my_j))) ++rank;
+        }
+        const int64_t o = (int64_t)i * P.k;
+        if (elig && rank < P.k) { P.top_idx[o + rank] = my_j; P.top_val[o + rank] = my_s; }
+        for (int z = n_el + lane; z < P.k; z += 32) { P.top_idx[o + z] = -1; P.top_val[o + z] = 0.0; }
+        const double nx = P.x_norm[i], ex = P.x_err[i];
+        double m = __dmul_ru(ex, Ny);
+        m = __dadd_ru(m, __dmul_ru(nx, Ey));
+        m = __dadd_ru(m, __dmul_ru(ex, Ey));
+        m = __dadd_ru(m, __dmul_ru(__dmul_ru(P.gamma, nx), Ny));
+        m = __dadd_ru(m, __dmul_ru(__dmul_ru(2.0 * P.d_pad * 0x1p-53, __dadd_ru(nx, ex)), __dadd_ru(Ny, Ey)));
+        bool cert;
+        if (nc < P.kc) cert = m <= P.m_max;
+        else {
+            const double B = __dadd_ru(P.cand_val[(int64_t)i * P.kc + P.kc - 1], m);
+            cert = B <= P.thr;
+            if (!cert && n_el >= P.k) {
+                const unsigned km = __ballot_sync(FULL, elig && rank == P.k - 1);
+                cert = __shfl_sync(FULL, my_s, __ffs(km) - 1) > B;    // strict: a to-row scoring exactly B could tie and win on index
+            }
+        }
+        if (!cert && lane == 0) P.fb_rows[atomicAdd(P.fb_count, 1)] = i;
+    }
+}
+
+// lane-distributed sorted list of a warp: lane z holds slot z < k, key (score desc, index asc), empty slots (-1) at the end
+__device__ __forceinline__ void lane_list_insert(double &lv, int &li, double s, int j, int k, int lane) {
+    const bool before = lane < k && li >= 0 && (lv > s || (lv == s && li < j));
+    const int pos = __popc(__ballot_sync(FULL, before));
+    if (pos >= k) return;
+    const double uv = __shfl_up_sync(FULL, lv, 1); const int ui = __shfl_up_sync(FULL, li, 1);
+    if (lane > pos) { lv = uv; li = ui; }
+    else if (lane == pos) { lv = s; li = j; }
+}
+__device__ __forceinline__ bool lane_list_takes(double kv, int ki, double s, int j) { return ki < 0 || s > kv || (s == kv && j < ki); }
+
+constexpr int FB_WARPS = 8, FB_CAP_ROWS = 2048, FB_MAX_SPLITS = 64, FB_ROWS_PER_SPLIT = 512;
+static int fb_splits(int n_to) { return max(1, min(FB_MAX_SPLITS, (n_to + FB_ROWS_PER_SPLIT - 1) / FB_ROWS_PER_SPLIT)); }
+
+struct FallbackParams {
+    const double *x, *y; int n_to, d_pad, k; double thr; int self_match; long long from_base, to_base;
+    const int32_t *fb_rows; const int32_t *fb_count; int n_splits, cap;
+    double *ws_val; int32_t *ws_idx; int32_t *ws_done; int32_t *top_idx; double *top_val;
+};
+
+// Brute-force canonical top-k over every to-row for the rows listed by exact_rescore_kernel (count read on the device).
+// Work item = (listed row, to-range split): the first `cap` listed rows are split n_splits ways, the CTA that finishes a
+// row's last split merges the partial lists; rows beyond `cap` are one item each over the whole to-range.
+__global__ void __launch_bounds__(FB_WARPS * 32) exact_fallback_kernel(const FallbackParams P) {
+    __shared__ double s_v[FB_WARPS][32];
+    __shared__ int s_i[FB_WARPS][32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int cnt = *P.fb_count;
+    const int n_split_rows = min(cnt, P.cap);
+    const long long n_split_items = (long long)n_split_rows * P.n_splits;
+    const long long n_items = n_split_items + (cnt - n_split_rows);
+    const int chunk = (P.n_to + P.n_splits - 1) / P.n_splits;
+    for (long long u = blockIdx.x; u < n_items; u += gridDim.x) {
+        int p, sp, lo, hi;
+        if (u < n_split_items) { p = (int)(u / P.n_splits); sp = (int)(u % P.n_splits); lo = sp * chunk; hi = min(P.n_to, lo + chunk); }
+        else { p = P.cap + (int)(u - n_split_items); sp = -1; lo = 0; hi = P.n_to; }
+        const int i = P.fb_rows[p];
+        const double *xr = P.x + (int64_t)i * P.d_pad;
+        const long long self_j = P.from_base + i - P.to_base;
+        double lv = 0.0, kv = 0.0; int li = -1, ki = -1;
+        for (int j = lo + warp; j < hi; j += FB_WARPS) {
+            const double *yr[1] = {P.y + (int64_t)j * P.d_pad}; double s[1];
+            warp_dot_canon<1>(xr, yr, P.d_pad, lane, s);
+            if (!(s[0] > P.thr) || (P.self_match && (long long)j == self_j)) continue;
+            const int gj = (int)(P.to_base + j);
+            if (!lane_list_takes(kv, ki, s[0], gj)) continue;
+            lane_list_insert(lv, li, s[0], gj, P.k, lane);
+            kv = __shfl_sync(FULL, lv, P.k - 1); ki = __shfl_sync(FULL, li, P.k - 1);
+        }
+        s_v[warp][lane] = lv; s_i[warp][lane] = li;
+        __syncthreads();
+        if (warp == 0) {
+            for (int w = 1; w < FB_WARPS; ++w)
+                for (int z = 0; z < P.k; ++z) {
+                    const int oj = s_i[w][z]; const double ov = s_v[w][z];
+                    if (oj < 0 || !lane_list_takes(kv, ki, ov, oj)) break;      // sorted: the rest of this list loses too
+                    lane_list_insert(lv, li, ov, oj, P.k, lane);
+                    kv = __shfl_sync(FULL, lv, P.k - 1); ki = __shfl_sync(FULL, li, P.k - 1);
+                }
+            bool write = sp < 0;
+            if (!write) {
+                const int64_t o = ((int64_t)p * P.n_splits + sp) * P.k;
+                if (lane < P.k) { P.ws_val[o + lane] = lv; P.ws_idx[o + lane] = li; }
+                __threadfence();
+                int last = 0;
+                if (lane == 0) last = atomicAdd(&P.ws_done[p], 1) == P.n_splits - 1;
+                write = __shfl_sync(FULL, last, 0) != 0;
+                if (write) {                                                   // every split of row p is in ws: merge them
+                    __threadfence();
+                    li = -1; ki = -1;
+                    for (int q = 0; q < P.n_splits; ++q)
+                        for (int z = 0; z < P.k; ++z) {
+                            const int64_t oq = ((int64_t)p * P.n_splits + q) * P.k + z;
+                            const int oj = __ldcg(P.ws_idx + oq); const double ov = __ldcg(P.ws_val + oq);
+                            if (oj < 0 || !lane_list_takes(kv, ki, ov, oj)) break;
+                            lane_list_insert(lv, li, ov, oj, P.k, lane);
+                            kv = __shfl_sync(FULL, lv, P.k - 1); ki = __shfl_sync(FULL, li, P.k - 1);
+                        }
+                }
+            }
+            if (write && lane < P.k) {
+                P.top_idx[(int64_t)i * P.k + lane] = li;
+                P.top_val[(int64_t)i * P.k + lane] = li >= 0 ? lv : 0.0;
+            }
+        }
+        __syncthreads();
+    }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
                                   CUtensorMapFloatOOBfill);
 
-static int make_map(EncodeTiledFn enc, CUtensorMap *m, const void *base, int n_rows, int d, int box_rows) {
+static int make_map(EncodeTiledFn enc, CUtensorMap *m, const void *base, int n_rows, int d, int box_rows, CUtensorMapDataType dt) {
     cuuint64_t dims[2] = {(cuuint64_t)d, (cuuint64_t)n_rows};
     cuuint64_t strides[1] = {(cuuint64_t)d * 2};
     cuuint32_t box[2] = {(cuuint32_t)DK, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = enc(m, dt, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return 1; }
     return 0;
 }
 
-template <int KMAX, bool MCAST>
-static int dense_launch(EncodeTiledFn enc, const void *x_bf16, const void *y_bf16, DenseParams P, int sms, cudaStream_t st) {
+template <int KMAX, bool MCAST, bool F16>
+static int dense_launch(EncodeTiledFn enc, const void *x_op, const void *y_op, DenseParams P, int sms, cudaStream_t st) {
+    const CUtensorMapDataType dt = F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     CUtensorMap mx, my;
-    if (make_map(enc, &mx, x_bf16, P.n_from, P.d, DM)) return 1;
-    if (make_map(enc, &my, y_bf16, P.n_to, P.d, MCAST ? DN / 2 : DN)) return 1;
+    if (make_map(enc, &mx, x_op, P.n_from, P.d, DM, dt)) return 1;
+    if (make_map(enc, &my, y_op, P.n_to, P.d, MCAST ? DN / 2 : DN, dt)) return 1;
     const int G = MCAST ? 2 : 1;
     int units = (P.n_mblocks + G - 1) / G * P.n_splits; if (units > sms / G) units = sms / G;
-    auto kern = dense_cos_topk_kernel<KMAX, MCAST>;
+    auto kern = dense_cos_topk_kernel<KMAX, MCAST, F16>;
     PFZ_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DENSE_SMEM));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(G * units)); cfg.blockDim = dim3(DENSE_THREADS); cfg.dynamicSmemBytes = DENSE_SMEM; cfg.stream = st;
@@ -315,6 +564,43 @@ static int dense_launch(EncodeTiledFn enc, const void *x_bf16, const void *y_bf1
     PFZ_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, mx, my, P));
     PFZ_LAUNCH_OK();
     return 0;
+}
+
+// shared by the bf16 and fp16 entry points: validation, launch shape, KMAX dispatch; the candidate threshold is min_sim
+template <bool F16>
+static int dense_topk_any(const char *fn, const void *x_op, const void *y_op, int32_t n_from, int32_t n_to, int32_t d, int32_t k, float min_sim,
+                          int32_t self_match, int64_t from_index_base, int64_t to_index_base, int32_t n_splits, int32_t *top_idx, double *top_val,
+                          void *stream) {
+    PFZ_REQUIRE(k >= 1 && k <= 32, "%s: k=%d unsupported (1..32)", fn, k);
+    PFZ_REQUIRE(d >= 8 && d % 8 == 0, "%s: d=%d must be a multiple of 8 (16-byte row pitch for TMA)", fn, d);
+    PFZ_REQUIRE(((uintptr_t)x_op % 16) == 0 && ((uintptr_t)y_op % 16) == 0, "%s: operands must be 16-byte aligned", fn);
+    if (n_from <= 0) return 0;
+    PFZ_REQUIRE(n_to > 0, "%s: empty to-matrix", fn);
+    static EncodeTiledFn enc = nullptr;
+    if (!enc) {
+        void *f = nullptr; cudaDriverEntryPointQueryResult qres;
+        PFZ_CUDA_OK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qres));
+        PFZ_REQUIRE(f && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available in this driver");
+        enc = (EncodeTiledFn)f;
+    }
+    const char *env2 = getenv("PFZ_K4_2CTA");                   // CTA pairs sharing the to-tile through TMA multicast (half the to-operand
+    const bool two_cta = env2 ? atoi(env2) != 0 : true;         // traffic per SM); 0 = one CTA per row block
+    DenseParams P;
+    P.n_from = n_from; P.n_to = n_to; P.d = d; P.k = k; P.min_sim = min_sim; P.self_match = self_match;
+    P.from_base = from_index_base; P.to_base = to_index_base;
+    P.n_mblocks = (n_from + DM - 1) / DM; P.n_ntiles = (n_to + DN - 1) / DN;
+    PFZ_REQUIRE(n_splits >= 1 && n_splits <= P.n_ntiles, "%s: n_splits %d out of range (1..%d)", fn, n_splits, P.n_ntiles);
+    P.n_splits = n_splits; P.top_idx = top_idx; P.top_val = top_val;
+    int dev = 0, sms = 0;
+    PFZ_CUDA_OK(cudaGetDevice(&dev));
+    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    cudaStream_t st = as_stream(stream);
+#define PFZ_DENSE_LAUNCH(KM) (two_cta ? dense_launch<KM, true, F16>(enc, x_op, y_op, P, sms, st) : dense_launch<KM, false, F16>(enc, x_op, y_op, P, sms, st))
+    if (k <= 4) return PFZ_DENSE_LAUNCH(4);
+    if (k <= 10) return PFZ_DENSE_LAUNCH(10);
+    if (k <= 16) return PFZ_DENSE_LAUNCH(16);
+    return PFZ_DENSE_LAUNCH(32);
+#undef PFZ_DENSE_LAUNCH
 }
 
 }  // namespace pfz
@@ -337,35 +623,79 @@ int pfz_rows_to_bf16(const void *x, int32_t is_f64, int64_t ld, int32_t n_rows, 
 int pfz_dense_cos_topk(const void *x_bf16, const void *y_bf16, int32_t n_from, int32_t n_to, int32_t d, int32_t k, double min_similarity,
                        int32_t self_match, int64_t from_index_base, int64_t to_index_base, int32_t n_splits, int32_t *top_idx, double *top_val,
                        void *stream) {
-    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_dense_cos_topk: k=%d unsupported (1..32)", k);
-    PFZ_REQUIRE(d >= 8 && d % 8 == 0, "pfz_dense_cos_topk: d=%d must be a multiple of 8 (16-byte row pitch for TMA)", d);
-    PFZ_REQUIRE(((uintptr_t)x_bf16 % 16) == 0 && ((uintptr_t)y_bf16 % 16) == 0, "pfz_dense_cos_topk: operands must be 16-byte aligned");
-    if (n_from <= 0) return 0;
-    PFZ_REQUIRE(n_to > 0, "pfz_dense_cos_topk: empty to-matrix");
-    static EncodeTiledFn enc = nullptr;
-    if (!enc) {
-        void *fn = nullptr; cudaDriverEntryPointQueryResult qres;
-        PFZ_CUDA_OK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-        PFZ_REQUIRE(fn && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available in this driver");
-        enc = (EncodeTiledFn)fn;
-    }
-    const char *env2 = getenv("PFZ_K4_2CTA");                   // CTA pairs sharing the to-tile through TMA multicast (half the to-operand
-    const bool two_cta = env2 ? atoi(env2) != 0 : true;         // traffic per SM); 0 = one CTA per row block
-    DenseParams P;
-    P.n_from = n_from; P.n_to = n_to; P.d = d; P.k = k; P.min_sim = (float)min_similarity; P.self_match = self_match;
-    P.from_base = from_index_base; P.to_base = to_index_base;
-    P.n_mblocks = (n_from + DM - 1) / DM; P.n_ntiles = (n_to + DN - 1) / DN;
-    PFZ_REQUIRE(n_splits >= 1 && n_splits <= P.n_ntiles, "pfz_dense_cos_topk: n_splits %d out of range (1..%d)", n_splits, P.n_ntiles);
-    P.n_splits = n_splits; P.top_idx = top_idx; P.top_val = top_val;
-    int dev = 0, sms = 0;
-    PFZ_CUDA_OK(cudaGetDevice(&dev));
-    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    return dense_topk_any<false>("pfz_dense_cos_topk", x_bf16, y_bf16, n_from, n_to, d, k, (float)min_similarity, self_match, from_index_base,
+                                 to_index_base, n_splits, top_idx, top_val, stream);
+}
+
+int pfz_rows_prep_exact(const void *x, int32_t is_f64, int64_t ld, int32_t n_rows, int32_t d, int32_t d_pad, double *out_f64, void *out_f16,
+                        double *norm16, double *err16, double *maxima, void *stream) {
+    PFZ_REQUIRE(d_pad >= d && d_pad % 8 == 0, "pfz_rows_prep_exact: d_pad %d must be >= d and a multiple of 8", d_pad);
     cudaStream_t st = as_stream(stream);
-#define PFZ_DENSE_LAUNCH(KM) (two_cta ? dense_launch<KM, true>(enc, x_bf16, y_bf16, P, sms, st) : dense_launch<KM, false>(enc, x_bf16, y_bf16, P, sms, st))
-    if (k <= 4) return PFZ_DENSE_LAUNCH(4);
-    if (k <= 10) return PFZ_DENSE_LAUNCH(10);
-    if (k <= 16) return PFZ_DENSE_LAUNCH(16);
-    return PFZ_DENSE_LAUNCH(32);
-#undef PFZ_DENSE_LAUNCH
+    if (maxima) PFZ_CUDA_OK(cudaMemsetAsync(maxima, 0, 2 * sizeof(double), st));
+    if (n_rows <= 0) return 0;
+    int grid = (n_rows + 7) / 8; if (grid > SM_COUNT * 16) grid = SM_COUNT * 16;
+    unsigned long long *mx = (unsigned long long *)maxima;
+    if (is_f64) rows_prep_exact_kernel<double><<<grid, 256, 0, st>>>((const double *)x, ld, n_rows, d, d_pad, out_f64, (__half *)out_f16, norm16, err16, mx);
+    else        rows_prep_exact_kernel<float><<<grid, 256, 0, st>>>((const float *)x, ld, n_rows, d, d_pad, out_f64, (__half *)out_f16, norm16, err16, mx);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
+int pfz_dense_cos_topk_f16(const void *x_f16, const void *y_f16, int32_t n_from, int32_t n_to, int32_t d, int32_t k, double min_similarity,
+                           int32_t self_match, int64_t from_index_base, int64_t to_index_base, int32_t n_splits, int32_t *top_idx, double *top_val,
+                           void *stream) {
+    // t_f: the largest float <= min_similarity - M_max(d)
+    const double t = nextafter(min_similarity - exact_margin_max(d), -INFINITY);
+    float tf = (float)t;
+    if ((double)tf > t) tf = nextafterf(tf, -INFINITY);
+    return dense_topk_any<true>("pfz_dense_cos_topk_f16", x_f16, y_f16, n_from, n_to, d, k, tf, self_match, from_index_base, to_index_base,
+                                n_splits, top_idx, top_val, stream);
+}
+
+int pfz_dense_exact_rescore(const double *x_f64, const double *y_f64, int32_t n_from, int32_t n_to, int32_t d_pad, int32_t k, int32_t k_cand,
+                            const int32_t *cand_idx, const double *cand_val, const double *x_norm16, const double *x_err16, const double *y_maxima,
+                            double min_similarity, int32_t self_match, int64_t from_index_base, int64_t to_index_base, int32_t *top_idx,
+                            double *top_val, int32_t *fb_rows, int32_t *fb_count, void *stream) {
+    PFZ_REQUIRE(k >= 1 && k <= 32 && k_cand >= k && k_cand <= 32, "pfz_dense_exact_rescore: need 1 <= k (%d) <= k_cand (%d) <= 32", k, k_cand);
+    PFZ_REQUIRE(d_pad >= 8 && d_pad % 8 == 0, "pfz_dense_exact_rescore: d_pad=%d must be a multiple of 8", d_pad);
+    cudaStream_t st = as_stream(stream);
+    PFZ_CUDA_OK(cudaMemsetAsync(fb_count, 0, sizeof(int32_t), st));
+    if (n_from <= 0) return 0;
+    PFZ_REQUIRE(n_to > 0, "pfz_dense_exact_rescore: empty to-matrix");
+    ExactParams P;
+    P.x = x_f64; P.y = y_f64; P.n_from = n_from; P.n_to = n_to; P.d_pad = d_pad; P.k = k; P.kc = k_cand;
+    P.thr = min_similarity; P.gamma = exact_gamma(d_pad); P.m_max = exact_margin_max(d_pad); P.self_match = self_match;
+    P.from_base = from_index_base; P.to_base = to_index_base;
+    P.cand_idx = cand_idx; P.cand_val = cand_val; P.x_norm = x_norm16; P.x_err = x_err16; P.y_max = y_maxima;
+    P.top_idx = top_idx; P.top_val = top_val; P.fb_rows = fb_rows; P.fb_count = fb_count;
+    int grid = (n_from + 7) / 8; if (grid > SM_COUNT * 16) grid = SM_COUNT * 16;
+    exact_rescore_kernel<<<grid, 256, 0, st>>>(P);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
+int64_t pfz_dense_exact_fallback_ws_bytes(int32_t n_from, int32_t n_to, int32_t k) {
+    const int64_t cap = n_from < FB_CAP_ROWS ? (n_from > 0 ? n_from : 1) : FB_CAP_ROWS;
+    return cap * fb_splits(n_to) * (int64_t)(k > 0 ? k : 1) * 12 + cap * 4 + 256;
+}
+
+int pfz_dense_exact_fallback(const double *x_f64, const double *y_f64, int32_t n_from, int32_t n_to, int32_t d_pad, int32_t k, double min_similarity,
+                             int32_t self_match, int64_t from_index_base, int64_t to_index_base, const int32_t *fb_rows, const int32_t *fb_count,
+                             int32_t *top_idx, double *top_val, void *ws, void *stream) {
+    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_dense_exact_fallback: k=%d unsupported (1..32)", k);
+    if (n_from <= 0) return 0;
+    PFZ_REQUIRE(n_to > 0, "pfz_dense_exact_fallback: empty to-matrix");
+    cudaStream_t st = as_stream(stream);
+    FallbackParams P;
+    P.x = x_f64; P.y = y_f64; P.n_to = n_to; P.d_pad = d_pad; P.k = k; P.thr = min_similarity; P.self_match = self_match;
+    P.from_base = from_index_base; P.to_base = to_index_base; P.fb_rows = fb_rows; P.fb_count = fb_count;
+    P.n_splits = fb_splits(n_to); P.cap = n_from < FB_CAP_ROWS ? n_from : FB_CAP_ROWS;
+    const int64_t n_part = (int64_t)P.cap * P.n_splits * k;
+    P.ws_val = (double *)ws; P.ws_idx = (int32_t *)(P.ws_val + n_part); P.ws_done = P.ws_idx + n_part;
+    P.top_idx = top_idx; P.top_val = top_val;
+    PFZ_CUDA_OK(cudaMemsetAsync(P.ws_done, 0, (size_t)P.cap * sizeof(int32_t), st));
+    exact_fallback_kernel<<<SM_COUNT * 4, FB_WARPS * 32, 0, st>>>(P);
+    PFZ_LAUNCH_OK();
+    return 0;
 }
 }

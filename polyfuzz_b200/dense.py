@@ -1,11 +1,13 @@
 """K4 host driver: dense cosine top-k of pre-computed embeddings on the tensor cores (include/pfz.h,
 pfz_rows_to_bf16 + pfz_dense_cos_topk).  Inputs are rounded to bf16 (after l2 normalisation in fp32);
-products accumulate in fp32 (wgmma register accumulators); the ranking key is (score desc, index asc) on those fp32 values."""
+products accumulate in fp32 (wgmma register accumulators); the ranking key is (score desc, index asc) on those fp32 values.
+The exact mode (stage_exact + dense_topk_exact) returns the canonical fp64 top-k instead: an fp16 tensor-core filter pass,
+fp64 re-scoring of its candidates with a per-row certificate, and a brute-force fp64 pass for the rows not certified."""
 import numpy as np
 import torch
 
 from . import _lib
-from .engine import _dev, _p, _stream, topk_merge
+from .engine import _dev, _p, _stream, _ws, topk_merge
 
 SM_COUNT = 132                     # H100 SXM
 
@@ -54,3 +56,119 @@ def dense_topk(x_bf16, y_bf16, k, min_similarity=0.0, self_match=False, from_ind
     if n_splits > 1:
         return topk_merge(ti, tv, k)
     return ti[0], tv[0]
+
+
+# ---- exact mode (Embeddings(precision="fp64")): the canonical fp64 top-k, bit for bit (DESIGN.md 2 and 4.6) ----------------
+
+class ExactRows:
+    """One side staged for the exact mode: canonical l2-normalised fp64 rows `f64` and their fp16 rounding `f16` (both
+    [n, d_pad], zero-padded), per-row upper bounds `norm16` >= ||f16 row|| and `err16` >= ||f64 row - f16 row||, and `maxima`
+    (float64[2], on the device) = the largest of each."""
+    __slots__ = ("f64", "f16", "norm16", "err16", "maxima")
+
+    @property
+    def n(self):
+        return self.f64.shape[0]
+
+    @property
+    def d_pad(self):
+        return self.f64.shape[1]
+
+
+def stage_exact(x):
+    """ndarray / tensor [n, d] (float32/float64) -> ExactRows on the device (pfz_rows_prep_exact).  fp32 inputs widen exactly."""
+    dev = _dev()
+    if isinstance(x, np.ndarray):
+        if x.dtype not in (np.float32, np.float64):
+            x = x.astype(np.float64)
+        t = torch.from_numpy(np.ascontiguousarray(x)).to(dev)
+    else:
+        t = x.to(dev)
+        if t.dtype not in (torch.float32, torch.float64):
+            t = t.double()
+        t = t.contiguous()
+    if t.dim() != 2:
+        raise ValueError("embeddings must be a 2-D array [n, d]")
+    n, d = t.shape
+    d_pad = max(8, (d + 7) // 8 * 8)
+    rows = max(n, 1)
+    s = ExactRows()
+    s.f64 = torch.empty((rows, d_pad), dtype=torch.float64, device=dev)
+    s.f16 = torch.empty((rows, d_pad), dtype=torch.float16, device=dev)
+    s.norm16 = torch.empty(rows, dtype=torch.float64, device=dev)
+    s.err16 = torch.empty(rows, dtype=torch.float64, device=dev)
+    s.maxima = torch.empty(2, dtype=torch.float64, device=dev)
+    _lib.call("pfz_rows_prep_exact", _p(t), int(t.dtype == torch.float64), int(t.stride(0)) if n else d, n, d, d_pad,
+              _p(s.f64), _p(s.f16), _p(s.norm16), _p(s.err16), _p(s.maxima), _stream())
+    s.f64, s.f16, s.norm16, s.err16 = s.f64[:n], s.f16[:n], s.norm16[:n], s.err16[:n]
+    return s
+
+
+def k_cand_for(k):
+    """Filter candidates per row for a top-k (DESIGN.md 4.6): the largest list of the kernel instantiation (KMAX 10 / 16 / 32)
+    that holds about 2k + 4.  The KMAX = 32 instantiation spills registers and filtered C4 5.5x slower than KMAX = 16, so k up
+    to 12 takes 16 candidates (C4, k = 10: 0.02 % of the rows then need the fallback)."""
+    k = int(k)
+    return 10 if k <= 3 else 16 if k <= 12 else 32
+
+
+def candidates_f16(xs, ys, k_cand, min_similarity=0.0, self_match=False, from_index_base=0, to_index_base=0, n_splits=None):
+    """Filter pass of the exact mode (pfz_dense_cos_topk_f16, + pfz_topk_merge over splits): per from-row the k_cand best
+    fp32 scores of fp16(x~) . fp16(y~) above min_similarity minus the a-priori margin.  Returns (idx int32, val float64)."""
+    dev = _dev()
+    n_from, d_pad = xs.f16.shape
+    n_to = ys.n
+    n_mblocks = (n_from + 127) // 128
+    n_ntiles = (n_to + 127) // 128
+    if n_splits is None:
+        n_splits = max(1, min(n_ntiles, (2 * SM_COUNT + n_mblocks - 1) // n_mblocks))
+    n_splits = max(1, min(int(n_splits), n_ntiles))
+    ti = torch.empty((n_splits, n_from, k_cand), dtype=torch.int32, device=dev)
+    tv = torch.empty((n_splits, n_from, k_cand), dtype=torch.float64, device=dev)
+    _lib.call("pfz_dense_cos_topk_f16", _p(xs.f16), _p(ys.f16), n_from, n_to, d_pad, k_cand, float(min_similarity), int(bool(self_match)),
+              int(from_index_base), int(to_index_base), n_splits, _p(ti), _p(tv), _stream())
+    if n_splits > 1:
+        return topk_merge(ti, tv, k_cand)
+    return ti[0], tv[0]
+
+
+def exact_rescore(xs, ys, cand_idx, cand_val, k, min_similarity=0.0, self_match=False, from_index_base=0, to_index_base=0):
+    """Canonical fp64 top-k of each row's filter candidates and its certificate (pfz_dense_exact_rescore).
+    Returns (idx, val, fb_rows, fb_count): fb_rows[:fb_count] are the rows left to exact_fallback."""
+    dev = _dev()
+    n_from = xs.n
+    idx = torch.empty((n_from, k), dtype=torch.int32, device=dev)
+    val = torch.empty((n_from, k), dtype=torch.float64, device=dev)
+    fb_rows = torch.empty(max(n_from, 1), dtype=torch.int32, device=dev)
+    fb_count = torch.empty(1, dtype=torch.int32, device=dev)
+    _lib.call("pfz_dense_exact_rescore", _p(xs.f64), _p(ys.f64), n_from, ys.n, xs.d_pad, k, int(cand_idx.shape[1]), _p(cand_idx.contiguous()),
+              _p(cand_val.contiguous()), _p(xs.norm16), _p(xs.err16), _p(ys.maxima), float(min_similarity), int(bool(self_match)),
+              int(from_index_base), int(to_index_base), _p(idx), _p(val), _p(fb_rows), _p(fb_count), _stream())
+    return idx, val, fb_rows, fb_count
+
+
+def exact_fallback(xs, ys, idx, val, fb_rows, fb_count, min_similarity=0.0, self_match=False, from_index_base=0, to_index_base=0):
+    """Canonical top-k over every to-row for the listed rows, written into idx / val in place (pfz_dense_exact_fallback)."""
+    n_from, k = idx.shape
+    ws = _ws(_lib.load().pfz_dense_exact_fallback_ws_bytes(n_from, ys.n, k))
+    _lib.call("pfz_dense_exact_fallback", _p(xs.f64), _p(ys.f64), n_from, ys.n, xs.d_pad, k, float(min_similarity), int(bool(self_match)),
+              int(from_index_base), int(to_index_base), _p(fb_rows), _p(fb_count), _p(idx), _p(val), _p(ws), _stream())
+
+
+def dense_topk_exact(xs, ys, k, min_similarity=0.0, self_match=False, from_index_base=0, to_index_base=0, n_splits=None, k_cand=None):
+    """Canonical fp64 cosine top-k of two ExactRows (stage_exact).  Returns (idx int32[n_from,k] global to-indices or -1,
+    val float64[n_from,k], fallback row count int32[1] on the device); no host synchronisation."""
+    dev = _dev()
+    k = int(k)
+    if not 1 <= k <= 32:
+        raise NotImplementedError("dense top_n is limited to 32 per call")
+    if xs.d_pad != ys.d_pad:
+        raise ValueError(f"embedding widths differ: {xs.d_pad} vs {ys.d_pad} (padded)")
+    if xs.n == 0:
+        return (torch.empty((0, k), dtype=torch.int32, device=dev), torch.empty((0, k), dtype=torch.float64, device=dev),
+                torch.zeros(1, dtype=torch.int32, device=dev))
+    kc = max(k, min(32, int(k_cand) if k_cand else k_cand_for(k)))
+    ci, cv = candidates_f16(xs, ys, kc, min_similarity, self_match, from_index_base, to_index_base, n_splits)
+    idx, val, fb_rows, fb_count = exact_rescore(xs, ys, ci, cv, k, min_similarity, self_match, from_index_base, to_index_base)
+    exact_fallback(xs, ys, idx, val, fb_rows, fb_count, min_similarity, self_match, from_index_base, to_index_base)
+    return idx, val, fb_count

@@ -1,7 +1,10 @@
 """Embeddings matcher -- drop-in for the pre-computed-vector path of polyfuzz.models.Embeddings
 (polyfuzz/models/_embeddings.py:87-135): dense cosine top-n on the tensor cores (K4).  The language-model
 embedders themselves (`_embed`, Flair / SBERT / ...) are out of scope (SURVEY.md section 2, rows 7-8): supply
-`embeddings_from` / `embeddings_to`, or an `embedding_method` callable `list[str] -> ndarray`."""
+`embeddings_from` / `embeddings_to`, or an `embedding_method` callable `list[str] -> ndarray`.
+
+precision="bf16" (default) ranks bf16-rounded rows on fp32 tensor-core accumulators; precision="fp64" returns the canonical
+fp64 cosine top-n bit for bit (DESIGN.md 2 and 4.6), the reference's sklearn-branch scores up to the last bits."""
 from typing import Callable, List
 
 import numpy as np
@@ -15,8 +18,11 @@ from ..distributed import get_comm, merge_topk_any, shard_bounds
 
 class Embeddings(BaseMatcher):
     def __init__(self, embedding_method: Callable = None, min_similarity: float = 0.75, top_n: int = 1,
-                 cosine_method: str = "sparse", model_id: str = None, distributed: bool = False):
+                 cosine_method: str = "sparse", model_id: str = None, distributed: bool = False, precision: str = "bf16"):
         super().__init__(model_id)
+        if precision not in ("bf16", "fp64"):
+            raise ValueError(f"precision {precision!r} unknown (bf16 | fp64)")
+        self.precision = precision
         self.type = "Embeddings"
         self.distributed = distributed      # torchrun: the to-matrix is row-sharded, one all-gather of per-shard top-k + merge
         self.embedding_method = embedding_method
@@ -48,19 +54,24 @@ class Embeddings(BaseMatcher):
         embeddings_from, embeddings_to = vec_from, vec_to
         top_n = clip_top_n(self.top_n, to_list)
         comm = get_comm() if self.distributed else None
-        x, _ = dense.to_bf16_rows(embeddings_from, normalize=True)
+        exact = self.precision == "fp64"
+        stage = dense.stage_exact if exact else (lambda e: dense.to_bf16_rows(e, normalize=True)[0])
+        x = stage(embeddings_from)
         lo = 0
         if comm is not None:                                  # this rank's contiguous row-block of the to-matrix (SURVEY.md 8e)
             lo, hi = shard_bounds(len(embeddings_to), comm.world_size, comm.rank)
-            y = dense.to_bf16_rows(embeddings_to[lo:hi], normalize=True)[0]
+            y = stage(embeddings_to[lo:hi])
         else:
-            y = x if embeddings_to is embeddings_from else dense.to_bf16_rows(embeddings_to, normalize=True)[0]
+            y = x if embeddings_to is embeddings_from else stage(embeddings_to)
         # `sparse` thresholds at min_similarity (polyfuzz/models/_utils.py:82); the reference's `sklearn` / `knn` branches
         # ignore it (_utils.py:59-70, 94-102) and blank scores below 0.001 afterwards: threshold 0 here
         if self.cosine_method not in ("sparse", "sklearn", "knn"):
             raise ValueError(f"cosine_method {self.cosine_method!r} unknown (sparse | sklearn | knn)")
         thr = self.min_similarity if self.cosine_method == "sparse" else 0.0
-        idx, val = dense.dense_topk(x, y, top_n, thr, self_match=to_list is None, to_index_base=lo)
+        if exact:                                             # each shard exact; the merge below then equals one GPU
+            idx, val, _ = dense.dense_topk_exact(x, y, top_n, thr, self_match=to_list is None, to_index_base=lo)
+        else:
+            idx, val = dense.dense_topk(x, y, top_n, thr, self_match=to_list is None, to_index_base=lo)
         if comm is not None:
             gi, gv = comm.all_gather_topk(idx.contiguous(), val.contiguous())
             idx, val = merge_topk_any(gi, gv, top_n)
