@@ -318,6 +318,43 @@ int pfz_dense_exact_fallback(const double *x_f64, const double *y_f64, int32_t n
                              const int32_t *fb_rows, const int32_t *fb_count, int32_t *top_idx, double *top_val, void *ws,
                              void *stream);
 
+/* K4 top_n > 32, both precisions (DESIGN.md 4.7): a bound per row from the UNMERGED lists of a top-16 call with n_splits >= 2k/16
+ * (pfz_dense_cos_topk, or pfz_dense_cos_topk_f16 in the exact mode), a threshold pass that appends every to-row scoring above the
+ * row's bound, and a per-row select.  Rows are processed in chunks by the caller, so the buffers below stay bounded.
+ *
+ * bound: row_thr (float[n_from]) from lists [n_lists][n_from][k_list] (global indices, -1 = empty).  exact == 0: the k-th best
+ *   score of the row's union; exact != 0: with f_k the k-th best filter score and M_i the row's margin (x_norm16 / x_err16 of
+ *   pfz_rows_prep_exact for these rows, y_maxima of the to-rows), tau = f_k - M_i and row_thr = tau - M_i (both rounded down)
+ *   when tau > min_similarity.  -inf when no bound exists (fewer than k entries, or tau <= min_similarity).               */
+int pfz_dense_topn_bound(const int32_t *list_idx, const double *list_val, int32_t n_lists, int32_t n_from, int32_t k_list,
+                         int32_t k, int32_t exact, const double *x_norm16, const double *x_err16, const double *y_maxima,
+                         int32_t d_pad, double min_similarity, float *row_thr, void *stream);
+
+/* threshold pass: K4 (bf16, or fp16 with the filter threshold t_f of pfz_dense_cos_topk_f16) appending every (global to-index,
+ * fp32 score as float64) with score >= row_thr[i] and score > min_similarity (t_f) to cand_idx / cand_val [n_from][cap] in
+ * no particular order.  cand_count (int32[n_from], zeroed by the callee) counts every such to-row, also past cap: a row with
+ * cand_count > cap must be re-run with a larger cap.  The diagonal is NOT excluded here (pfz_dense_topn_select does that).
+ * The bf16 scores are the same fp32 values pfz_dense_cos_topk ranks.                                                     */
+int pfz_dense_cos_cand(const void *x_bf16, const void *y_bf16, int32_t n_from, int32_t n_to, int32_t d, double min_similarity,
+                       const float *row_thr, int64_t to_index_base, int32_t n_splits, int32_t cap, int32_t *cand_idx,
+                       double *cand_val, int32_t *cand_count, void *stream);
+int pfz_dense_cos_cand_f16(const void *x_f16, const void *y_f16, int32_t n_from, int32_t n_to, int32_t d, double min_similarity,
+                           const float *row_thr, int64_t to_index_base, int32_t n_splits, int32_t cap, int32_t *cand_idx,
+                           double *cand_val, int32_t *cand_count, void *stream);
+
+/* exact mode: replaces each candidate's filter score by its canonical fp64 score.  Row r's from-row is
+ * x_f64[row_map ? row_map[r] : r]; y_f64 holds the to-rows of global index to_index_base + local row.                    */
+int pfz_dense_topn_exact_rescore(const double *x_f64, const double *y_f64, int32_t n_rows, int32_t d_pad, const int32_t *row_map,
+                                 int64_t to_index_base, int32_t cap, const int32_t *cand_idx, double *cand_val,
+                                 const int32_t *cand_count, void *stream);
+
+/* select: the top k of each row's min(cand_count, cap) candidates by (score desc, index asc), keeping score > min_similarity
+ * and, with self_match, dropping to-index from_index_base + output row; written to output row (row_map ? row_map[r] : r) of
+ * top_idx / top_val [..][k], empty slots (-1, 0.0).  Any k and any cap.                                                   */
+int pfz_dense_topn_select(const int32_t *cand_idx, const double *cand_val, const int32_t *cand_count, int32_t n_rows, int32_t cap,
+                          int32_t k, double min_similarity, int32_t self_match, int64_t from_index_base, const int32_t *row_map,
+                          int32_t *top_idx, double *top_val, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * K5  frame tail: top-k arrays -> the columns of the result frame (csrc/pfz_assemble.cu).
  * Replaces: polyfuzz/models/_utils.py:104-125 (the per-rank `[to_list[idx] ...]` gathers, the 3-decimal rounding of :102/:143

@@ -52,6 +52,11 @@ _PROTOS = {
                                 c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_dense_exact_fallback_ws_bytes": [c_i32, c_i32, c_i32],
     "pfz_dense_exact_fallback": [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    "pfz_dense_topn_bound": [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp, c_i32, c_f64, c_vp, c_vp],
+    "pfz_dense_cos_cand": [c_vp, c_vp, c_i32, c_i32, c_i32, c_f64, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp],
+    "pfz_dense_cos_cand_f16": [c_vp, c_vp, c_i32, c_i32, c_i32, c_f64, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp],
+    "pfz_dense_topn_exact_rescore": [c_vp, c_vp, c_i32, c_i32, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp],
+    "pfz_dense_topn_select": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp],
 }
 _RESTYPES = {"pfz_last_error": ctypes.c_char_p, "pfz_scan_ws_bytes": c_i64, "pfz_launch_count": c_i64, "pfz_spcos_block_ws_bytes": c_i64,
              "pfz_dense_exact_fallback_ws_bytes": c_i64}

@@ -109,6 +109,8 @@ struct DenseParams {
     int n_from, n_to, d; int k; float min_sim; int self_match; long long from_base, to_base;
     int n_splits; int n_mblocks; int n_ntiles;
     int32_t *top_idx; double *top_val;          // [n_splits][n_from][k]
+    // threshold epilogue only (appended, so the top-k instantiations read their fields at the same offsets)
+    const float *row_thr; int32_t *cand_cnt; int32_t *cand_idx; double *cand_val; int cap;   // [n_from], [n_from][cap]
 };
 
 // sorted insert into one row's top-k list; (kv, ki) tracks the k-th key, ki relative to to_base (-1 while not full)
@@ -124,8 +126,12 @@ __device__ __forceinline__ void topk_insert(float (&tv)[KMAX], int (&ti)[KMAX], 
     }
 }
 
-// F16: operands are fp16 instead of bf16 (the filter pass of the exact mode); nothing else differs
-template <int KMAX, bool MCAST, bool F16>
+// F16: operands are fp16 instead of bf16 (the filter pass of the exact mode); nothing else differs.
+// THRESH: the threshold epilogue of top_n > 32 (DESIGN.md 4.7) replaces the register top-k: every (j, score) with
+// score >= row_thr[i] and score > min_sim is appended to row i's candidate buffer (capacity cap; cand_cnt[i] keeps counting
+// past it).  The four threads of a quad agree on their offsets with shuffles, so a row takes one global atomic per tile.
+// The mainloop is the same code, so the scores are the same fp32 bits as the top-k instantiations'.
+template <int KMAX, bool MCAST, bool F16, bool THRESH = false>
 __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const __grid_constant__ CUtensorMap map_x,
                                                                           const __grid_constant__ CUtensorMap map_y, const DenseParams P) {
     constexpr int S = DSTAGES, G = MCAST ? 2 : 1;
@@ -198,6 +204,11 @@ __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const 
                 for (int q = 0; q < KMAX; ++q) { tv[h][q] = P.min_sim; ti[h][q] = -1; }
                 kv[h] = P.min_sim; ki[h] = -1;
             }
+            float rthr[2];
+            if constexpr (THRESH) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) rthr[h] = row0 + 8 * h < P.n_from ? P.row_thr[row0 + 8 * h] : INFINITY;
+            }
             for (int t = t_lo; t < t_hi; ++t) {
                 float acc[DN / 2];
                 int prev = -1;
@@ -221,8 +232,42 @@ __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const 
                 release(prev);
                 // accumulator layout: acc[4 j + 2 h + e] = (row0 + 8 h, column 8 j + 2 q4 + e of the tile)
                 const int colb = t * DN + 2 * q4;
+                if constexpr (THRESH) {
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = row0 + 8 * h;
+                        unsigned mask = 0u;
+#pragma unroll
+                        for (int q = 0; q < 32; ++q) {
+                            const int j = q >> 1;
+                            const float sc = acc[4 * j + 2 * h + (q & 1)];
+                            if (sc >= rthr[h] && sc > P.min_sim && colb + 8 * j + (q & 1) < P.n_to) mask |= 1u << q;
+                        }
+                        // quad prefix of the counts; lane 0 of the quad reserves the row's slots with one atomic
+                        const int cnt = __popc(mask);
+                        int incl = cnt;
+                        const int u1 = __shfl_up_sync(FULL, incl, 1, 4); if (q4 >= 1) incl += u1;
+                        const int u2 = __shfl_up_sync(FULL, incl, 2, 4); if (q4 >= 2) incl += u2;
+                        const int tot = __shfl_sync(FULL, incl, 3, 4);
+                        int base = 0;
+                        if (q4 == 0 && tot > 0) base = atomicAdd(P.cand_cnt + row, tot);
+                        int pos = __shfl_sync(FULL, base, 0, 4) + incl - cnt;
+                        while (mask) {
+                            const int q = __ffs(mask) - 1; mask &= mask - 1;
+                            float sc = 0.f;
+#pragma unroll
+                            for (int z = 0; z < 32; ++z) if (z == q) sc = acc[4 * (z >> 1) + 2 * h + (z & 1)];
+                            if (pos < P.cap) {
+                                const size_t o = (size_t)row * P.cap + pos;
+                                P.cand_idx[o] = (int)(P.to_base + colb + 8 * (q >> 1) + (q & 1));
+                                P.cand_val[o] = (double)sc;
+                            }
+                            ++pos;
+                        }
+                    }
+                }
+#pragma unroll
+                for (int h = 0; h < (THRESH ? 0 : 2); ++h) {              // the top-k epilogue
                     const long long self_col = P.from_base + row0 + 8 * h - P.to_base;   // local to-column of the diagonal
 #pragma unroll
                     for (int c = 0; c < DN / 128; ++c) {
@@ -251,7 +296,7 @@ __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const 
             }
             // the four threads of a quad hold disjoint column sets of the same two rows: k rounds of "best head wins"
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
+            for (int h = 0; h < (THRESH ? 0 : 2); ++h) {
                 const int row = row0 + 8 * h;
                 const size_t o = ((size_t)sp * P.n_from + row) * P.k;
 #pragma unroll
@@ -382,6 +427,16 @@ struct ExactParams {
     int32_t *top_idx; double *top_val; int32_t *fb_rows; int32_t *fb_count;
 };
 
+// M_i of from-row i (below): an upper bound on |fp32 filter score - canonical score| for every to-row
+__device__ __forceinline__ double exact_row_margin(double nx, double ex, double Ny, double Ey, double gamma, int d_pad) {
+    double m = __dmul_ru(ex, Ny);
+    m = __dadd_ru(m, __dmul_ru(nx, Ey));
+    m = __dadd_ru(m, __dmul_ru(ex, Ey));
+    m = __dadd_ru(m, __dmul_ru(__dmul_ru(gamma, nx), Ny));
+    m = __dadd_ru(m, __dmul_ru(__dmul_ru(2.0 * d_pad * 0x1p-53, __dadd_ru(nx, ex)), __dadd_ru(Ny, Ey)));
+    return m;
+}
+
 // One warp per from-row: canonical scores of the row's <= kc filter candidates (lane c holds candidate c), the exact top-k of
 // the eligible ones, and the certificate that no other to-row belongs in it.  With s_kc the kc-th filter score and
 //   M_i = e_x N_y + n_x E_y + e_x E_y + gamma n_x N_y + 2 d_pad 2^-53 (n_x + e_x)(N_y + E_y)   (rounded up)
@@ -422,12 +477,7 @@ __global__ void __launch_bounds__(256) exact_rescore_kernel(const ExactParams P)
         const int64_t o = (int64_t)i * P.k;
         if (elig && rank < P.k) { P.top_idx[o + rank] = my_j; P.top_val[o + rank] = my_s; }
         for (int z = n_el + lane; z < P.k; z += 32) { P.top_idx[o + z] = -1; P.top_val[o + z] = 0.0; }
-        const double nx = P.x_norm[i], ex = P.x_err[i];
-        double m = __dmul_ru(ex, Ny);
-        m = __dadd_ru(m, __dmul_ru(nx, Ey));
-        m = __dadd_ru(m, __dmul_ru(ex, Ey));
-        m = __dadd_ru(m, __dmul_ru(__dmul_ru(P.gamma, nx), Ny));
-        m = __dadd_ru(m, __dmul_ru(__dmul_ru(2.0 * P.d_pad * 0x1p-53, __dadd_ru(nx, ex)), __dadd_ru(Ny, Ey)));
+        const double m = exact_row_margin(P.x_norm[i], P.x_err[i], Ny, Ey, P.gamma, P.d_pad);
         bool cert;
         if (nc < P.kc) cert = m <= P.m_max;
         else {
@@ -531,6 +581,129 @@ __global__ void __launch_bounds__(FB_WARPS * 32) exact_fallback_kernel(const Fal
     }
 }
 
+// ---- top_n > 32 (DESIGN.md 4.7): bound from unmerged KMAX = 16 lists, threshold pass, select --------------------------------
+
+constexpr int SEL_THREADS = 256, SEL_PER = 8, SEL_TILE = SEL_THREADS * SEL_PER;
+
+struct SelectParams {
+    const int32_t *idx; const double *val; const int32_t *count;         // count NULL: every row has n_cand entries
+    int n_rows, n_cand; long long row_stride, seg_stride; int seg_len;  // entry e of row r: r row_stride + (e / seg_len) seg_stride + e % seg_len
+    const int32_t *row_map;                                             // output row of row r (NULL: r)
+    int k; double thr; int self_match; long long from_base;             // eligible: index >= 0, score > thr, not the diagonal
+    int32_t *top_idx; double *top_val;                                  // list mode: [output rows][k]
+    float *row_thr;                                                     // bound mode (non-NULL): per output row, instead of a list
+    int exact; double thr_bound; const double *x_norm, *x_err, *y_max; double gamma; int d_pad;
+};
+
+// One CTA per row: the rank of every eligible entry under (score desc, index asc) by counting the entries that rank before it;
+// entries are unique by index, so the ranks 0 .. n_el - 1 are distinct.  A batch of SEL_TILE entries sits in registers (SEL_PER
+// per thread) while the row streams through shared memory in tiles of SEL_TILE, so any count works; an entry stops counting
+// once its rank reaches k.  List mode writes the top k (empty slots (-1, 0.0)); bound mode writes the row threshold of the
+// threshold pass from the k-th entry (-inf when fewer than k entries are eligible, i.e. no bound: every score passes).
+__global__ void __launch_bounds__(SEL_THREADS) topn_select_kernel(const SelectParams P) {
+    __shared__ double s_v[SEL_TILE];
+    __shared__ int s_i[SEL_TILE];
+    __shared__ int s_nel;
+    const int tid = threadIdx.x;
+    for (int r = blockIdx.x; r < P.n_rows; r += gridDim.x) {
+        const int orow = P.row_map ? P.row_map[r] : r;
+        const int n = P.count ? min(P.count[r], P.n_cand) : P.n_cand;
+        const long long self_j = P.from_base + orow;
+        auto load = [&](int e, double &v, int &j) {
+            const long long o = (long long)r * P.row_stride + (long long)(e / P.seg_len) * P.seg_stride + e % P.seg_len;
+            j = P.idx[o]; v = P.val[o];
+            if (j < 0 || !(v > P.thr) || (P.self_match && (long long)j == self_j)) j = -1;
+        };
+        if (tid == 0) { s_nel = 0; if (P.row_thr) P.row_thr[orow] = -INFINITY; }
+        __syncthreads();
+        for (int b0 = 0; b0 < n; b0 += SEL_TILE) {
+            double ov[SEL_PER]; int oj[SEL_PER], rk[SEL_PER];
+            int mine = 0;
+#pragma unroll
+            for (int q = 0; q < SEL_PER; ++q) {
+                const int e = b0 + q * SEL_THREADS + tid;
+                ov[q] = 0.0; oj[q] = -1; rk[q] = 0;
+                if (e < n) load(e, ov[q], oj[q]);
+                mine += oj[q] >= 0;
+            }
+            if (mine) atomicAdd(&s_nel, mine);
+            for (int t0 = 0; t0 < n; t0 += SEL_TILE) {
+                const int tn = min(SEL_TILE, n - t0);
+                __syncthreads();
+                for (int z = tid; z < tn; z += SEL_THREADS) { double v; int j; load(t0 + z, v, j); s_v[z] = v; s_i[z] = j; }
+                __syncthreads();
+#pragma unroll
+                for (int q = 0; q < SEL_PER; ++q) {
+                    if (oj[q] < 0) continue;
+                    int c = rk[q];
+                    for (int z = 0; z < tn && c < P.k; ++z) {
+                        const int oz = s_i[z]; const double vz = s_v[z];
+                        c += oz >= 0 && (vz > ov[q] || (vz == ov[q] && oz < oj[q]));
+                    }
+                    rk[q] = c;
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < SEL_PER; ++q) {
+                if (oj[q] < 0 || rk[q] >= P.k) continue;
+                if (!P.row_thr) {
+                    const int64_t o = (int64_t)orow * P.k + rk[q];
+                    P.top_idx[o] = oj[q]; P.top_val[o] = ov[q];
+                } else if (rk[q] == P.k - 1) {
+                    float rt;
+                    if (!P.exact) rt = (float)ov[q];                       // an fp32 score: the threshold is the k-th score itself
+                    else {                                                 // tau = f_k - M_i; emit f >= tau - M_i when tau > thr
+                        const double m = exact_row_margin(P.x_norm[orow], P.x_err[orow], P.y_max[0], P.y_max[1], P.gamma, P.d_pad);
+                        const double tau = __dsub_rd(ov[q], m);
+                        rt = tau > P.thr_bound ? __double2float_rd(__dsub_rd(tau, m)) : -INFINITY;
+                    }
+                    P.row_thr[orow] = rt;
+                }
+            }
+        }
+        __syncthreads();
+        if (!P.row_thr)
+            for (int z = s_nel + tid; z < P.k; z += SEL_THREADS) { P.top_idx[(int64_t)orow * P.k + z] = -1; P.top_val[(int64_t)orow * P.k + z] = 0.0; }
+        __syncthreads();
+    }
+}
+
+struct CandRescoreParams {
+    const double *x, *y; int n_rows, d_pad, cap; long long to_base;
+    const int32_t *row_map; const int32_t *cand_idx; double *cand_val; const int32_t *count;
+};
+
+// exact mode: every candidate's filter score is replaced by its canonical fp64 score.  One warp per (row, 32 candidates).
+__global__ void __launch_bounds__(256) topn_exact_rescore_kernel(const CandRescoreParams P) {
+    constexpr int NC = 4;
+    const int lane = threadIdx.x & 31;
+    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = ((long long)gridDim.x * blockDim.x) >> 5;
+    const int slabs = (P.cap + 31) / 32;
+    const long long items = (long long)P.n_rows * slabs;
+    for (long long it = gw; it < items; it += nw) {
+        const int r = (int)(it / slabs), c0s = (int)(it % slabs) * 32;
+        const int n = min(P.count[r], P.cap);
+        if (c0s >= n) continue;
+        const int nc = min(32, n - c0s);
+        const double *xr = P.x + (int64_t)(P.row_map ? P.row_map[r] : r) * P.d_pad;
+        const size_t o = (size_t)r * P.cap + c0s;
+        const int my_j = lane < nc ? P.cand_idx[o + lane] : -1;
+        double my_s = 0.0;
+        for (int c0 = 0; c0 < nc; c0 += NC) {
+            const double *yr[NC]; double s[NC];
+#pragma unroll
+            for (int u = 0; u < NC; ++u) {
+                const int j = __shfl_sync(FULL, my_j, min(c0 + u, nc - 1));
+                yr[u] = P.y + ((int64_t)j - P.to_base) * P.d_pad;
+            }
+            warp_dot_canon<NC>(xr, yr, P.d_pad, lane, s);
+#pragma unroll
+            for (int u = 0; u < NC; ++u) if (lane == c0 + u) my_s = s[u];
+        }
+        if (lane < nc) P.cand_val[o + lane] = my_s;
+    }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
                                   CUtensorMapFloatOOBfill);
@@ -546,7 +719,7 @@ static int make_map(EncodeTiledFn enc, CUtensorMap *m, const void *base, int n_r
     return 0;
 }
 
-template <int KMAX, bool MCAST, bool F16>
+template <int KMAX, bool MCAST, bool F16, bool THRESH = false>
 static int dense_launch(EncodeTiledFn enc, const void *x_op, const void *y_op, DenseParams P, int sms, cudaStream_t st) {
     const CUtensorMapDataType dt = F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     CUtensorMap mx, my;
@@ -554,7 +727,7 @@ static int dense_launch(EncodeTiledFn enc, const void *x_op, const void *y_op, D
     if (make_map(enc, &my, y_op, P.n_to, P.d, MCAST ? DN / 2 : DN, dt)) return 1;
     const int G = MCAST ? 2 : 1;
     int units = (P.n_mblocks + G - 1) / G * P.n_splits; if (units > sms / G) units = sms / G;
-    auto kern = dense_cos_topk_kernel<KMAX, MCAST, F16>;
+    auto kern = dense_cos_topk_kernel<KMAX, MCAST, F16, THRESH>;
     PFZ_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DENSE_SMEM));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(G * units)); cfg.blockDim = dim3(DENSE_THREADS); cfg.dynamicSmemBytes = DENSE_SMEM; cfg.stream = st;
@@ -566,12 +739,10 @@ static int dense_launch(EncodeTiledFn enc, const void *x_op, const void *y_op, D
     return 0;
 }
 
-// shared by the bf16 and fp16 entry points: validation, launch shape, KMAX dispatch; the candidate threshold is min_sim
-template <bool F16>
-static int dense_topk_any(const char *fn, const void *x_op, const void *y_op, int32_t n_from, int32_t n_to, int32_t d, int32_t k, float min_sim,
-                          int32_t self_match, int64_t from_index_base, int64_t to_index_base, int32_t n_splits, int32_t *top_idx, double *top_val,
-                          void *stream) {
-    PFZ_REQUIRE(k >= 1 && k <= 32, "%s: k=%d unsupported (1..32)", fn, k);
+// shared by every K4 entry point: validation, tensor-map encoder, launch shape.  Sets *run = false when there is nothing to do.
+static int dense_prepare(const char *fn, const void *x_op, const void *y_op, int32_t n_from, int32_t n_to, int32_t d, int32_t n_splits,
+                         DenseParams &P, EncodeTiledFn &enc_out, bool &two_cta, int &sms, bool &run) {
+    run = false;
     PFZ_REQUIRE(d >= 8 && d % 8 == 0, "%s: d=%d must be a multiple of 8 (16-byte row pitch for TMA)", fn, d);
     PFZ_REQUIRE(((uintptr_t)x_op % 16) == 0 && ((uintptr_t)y_op % 16) == 0, "%s: operands must be 16-byte aligned", fn);
     if (n_from <= 0) return 0;
@@ -583,17 +754,32 @@ static int dense_topk_any(const char *fn, const void *x_op, const void *y_op, in
         PFZ_REQUIRE(f && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available in this driver");
         enc = (EncodeTiledFn)f;
     }
+    enc_out = enc;
     const char *env2 = getenv("PFZ_K4_2CTA");                   // CTA pairs sharing the to-tile through TMA multicast (half the to-operand
-    const bool two_cta = env2 ? atoi(env2) != 0 : true;         // traffic per SM); 0 = one CTA per row block
-    DenseParams P;
-    P.n_from = n_from; P.n_to = n_to; P.d = d; P.k = k; P.min_sim = min_sim; P.self_match = self_match;
-    P.from_base = from_index_base; P.to_base = to_index_base;
+    two_cta = env2 ? atoi(env2) != 0 : true;                    // traffic per SM); 0 = one CTA per row block
+    P = DenseParams{};
+    P.n_from = n_from; P.n_to = n_to; P.d = d;
     P.n_mblocks = (n_from + DM - 1) / DM; P.n_ntiles = (n_to + DN - 1) / DN;
     PFZ_REQUIRE(n_splits >= 1 && n_splits <= P.n_ntiles, "%s: n_splits %d out of range (1..%d)", fn, n_splits, P.n_ntiles);
-    P.n_splits = n_splits; P.top_idx = top_idx; P.top_val = top_val;
-    int dev = 0, sms = 0;
+    P.n_splits = n_splits;
+    int dev = 0;
     PFZ_CUDA_OK(cudaGetDevice(&dev));
     PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    run = true;
+    return 0;
+}
+
+// the bf16 and fp16 top-k entry points: KMAX dispatch; the candidate threshold is min_sim
+template <bool F16>
+static int dense_topk_any(const char *fn, const void *x_op, const void *y_op, int32_t n_from, int32_t n_to, int32_t d, int32_t k, float min_sim,
+                          int32_t self_match, int64_t from_index_base, int64_t to_index_base, int32_t n_splits, int32_t *top_idx, double *top_val,
+                          void *stream) {
+    PFZ_REQUIRE(k >= 1 && k <= 32, "%s: k=%d unsupported (1..32)", fn, k);
+    DenseParams P; EncodeTiledFn enc = nullptr; bool two_cta = true, run = false; int sms = 0;
+    if (dense_prepare(fn, x_op, y_op, n_from, n_to, d, n_splits, P, enc, two_cta, sms, run)) return 1;
+    if (!run) return 0;
+    P.k = k; P.min_sim = min_sim; P.self_match = self_match; P.from_base = from_index_base; P.to_base = to_index_base;
+    P.top_idx = top_idx; P.top_val = top_val;
     cudaStream_t st = as_stream(stream);
 #define PFZ_DENSE_LAUNCH(KM) (two_cta ? dense_launch<KM, true, F16>(enc, x_op, y_op, P, sms, st) : dense_launch<KM, false, F16>(enc, x_op, y_op, P, sms, st))
     if (k <= 4) return PFZ_DENSE_LAUNCH(4);
@@ -601,6 +787,30 @@ static int dense_topk_any(const char *fn, const void *x_op, const void *y_op, in
     if (k <= 16) return PFZ_DENSE_LAUNCH(16);
     return PFZ_DENSE_LAUNCH(32);
 #undef PFZ_DENSE_LAUNCH
+}
+
+// the bf16 and fp16 threshold-pass entry points (top_n > 32): appends to per-row candidate buffers, counters zeroed here
+template <bool F16>
+static int dense_cand_any(const char *fn, const void *x_op, const void *y_op, int32_t n_from, int32_t n_to, int32_t d, float min_sim,
+                          const float *row_thr, int64_t to_index_base, int32_t n_splits, int32_t cap, int32_t *cand_idx, double *cand_val,
+                          int32_t *cand_count, void *stream) {
+    PFZ_REQUIRE(cap >= 1, "%s: cap=%d must be >= 1", fn, cap);
+    DenseParams P; EncodeTiledFn enc = nullptr; bool two_cta = true, run = false; int sms = 0;
+    if (dense_prepare(fn, x_op, y_op, n_from, n_to, d, n_splits, P, enc, two_cta, sms, run)) return 1;
+    if (!run) return 0;
+    cudaStream_t st = as_stream(stream);
+    PFZ_CUDA_OK(cudaMemsetAsync(cand_count, 0, (size_t)n_from * sizeof(int32_t), st));
+    P.k = 1; P.min_sim = min_sim; P.self_match = 0; P.from_base = 0; P.to_base = to_index_base;
+    P.row_thr = row_thr; P.cand_cnt = cand_count; P.cand_idx = cand_idx; P.cand_val = cand_val; P.cap = cap;
+    return two_cta ? dense_launch<1, true, F16, true>(enc, x_op, y_op, P, sms, st) : dense_launch<1, false, F16, true>(enc, x_op, y_op, P, sms, st);
+}
+
+// t_f of the fp16 filter: the largest float <= min_similarity - M_max(d)
+static float filter_threshold(double min_similarity, int d) {
+    const double t = nextafter(min_similarity - exact_margin_max(d), -INFINITY);
+    float tf = (float)t;
+    if ((double)tf > t) tf = nextafterf(tf, -INFINITY);
+    return tf;
 }
 
 }  // namespace pfz
@@ -644,12 +854,69 @@ int pfz_rows_prep_exact(const void *x, int32_t is_f64, int64_t ld, int32_t n_row
 int pfz_dense_cos_topk_f16(const void *x_f16, const void *y_f16, int32_t n_from, int32_t n_to, int32_t d, int32_t k, double min_similarity,
                            int32_t self_match, int64_t from_index_base, int64_t to_index_base, int32_t n_splits, int32_t *top_idx, double *top_val,
                            void *stream) {
-    // t_f: the largest float <= min_similarity - M_max(d)
-    const double t = nextafter(min_similarity - exact_margin_max(d), -INFINITY);
-    float tf = (float)t;
-    if ((double)tf > t) tf = nextafterf(tf, -INFINITY);
-    return dense_topk_any<true>("pfz_dense_cos_topk_f16", x_f16, y_f16, n_from, n_to, d, k, tf, self_match, from_index_base, to_index_base,
-                                n_splits, top_idx, top_val, stream);
+    return dense_topk_any<true>("pfz_dense_cos_topk_f16", x_f16, y_f16, n_from, n_to, d, k, filter_threshold(min_similarity, d), self_match,
+                                from_index_base, to_index_base, n_splits, top_idx, top_val, stream);
+}
+
+int pfz_dense_cos_cand(const void *x_bf16, const void *y_bf16, int32_t n_from, int32_t n_to, int32_t d, double min_similarity,
+                       const float *row_thr, int64_t to_index_base, int32_t n_splits, int32_t cap, int32_t *cand_idx, double *cand_val,
+                       int32_t *cand_count, void *stream) {
+    return dense_cand_any<false>("pfz_dense_cos_cand", x_bf16, y_bf16, n_from, n_to, d, (float)min_similarity, row_thr, to_index_base, n_splits,
+                                 cap, cand_idx, cand_val, cand_count, stream);
+}
+
+int pfz_dense_cos_cand_f16(const void *x_f16, const void *y_f16, int32_t n_from, int32_t n_to, int32_t d, double min_similarity,
+                           const float *row_thr, int64_t to_index_base, int32_t n_splits, int32_t cap, int32_t *cand_idx, double *cand_val,
+                           int32_t *cand_count, void *stream) {
+    return dense_cand_any<true>("pfz_dense_cos_cand_f16", x_f16, y_f16, n_from, n_to, d, filter_threshold(min_similarity, d), row_thr,
+                                to_index_base, n_splits, cap, cand_idx, cand_val, cand_count, stream);
+}
+
+static int topn_select_launch(const SelectParams &P, cudaStream_t st) {
+    if (P.n_rows <= 0) return 0;
+    const int grid = P.n_rows < SM_COUNT * 8 ? P.n_rows : SM_COUNT * 8;
+    topn_select_kernel<<<grid, SEL_THREADS, 0, st>>>(P);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
+int pfz_dense_topn_bound(const int32_t *list_idx, const double *list_val, int32_t n_lists, int32_t n_from, int32_t k_list, int32_t k,
+                         int32_t exact, const double *x_norm16, const double *x_err16, const double *y_maxima, int32_t d_pad,
+                         double min_similarity, float *row_thr, void *stream) {
+    PFZ_REQUIRE(n_lists >= 1 && k_list >= 1 && k >= 1, "pfz_dense_topn_bound: need n_lists, k_list, k >= 1");
+    SelectParams P = {};
+    P.idx = list_idx; P.val = list_val; P.count = nullptr; P.n_rows = n_from; P.n_cand = n_lists * k_list;
+    P.row_stride = k_list; P.seg_len = k_list; P.seg_stride = (long long)n_from * k_list;
+    P.k = k; P.thr = -INFINITY; P.self_match = 0; P.row_thr = row_thr;
+    P.exact = exact; P.thr_bound = min_similarity; P.x_norm = x_norm16; P.x_err = x_err16; P.y_max = y_maxima;
+    P.gamma = exact_gamma(d_pad); P.d_pad = d_pad;
+    return topn_select_launch(P, as_stream(stream));
+}
+
+int pfz_dense_topn_exact_rescore(const double *x_f64, const double *y_f64, int32_t n_rows, int32_t d_pad, const int32_t *row_map,
+                                 int64_t to_index_base, int32_t cap, const int32_t *cand_idx, double *cand_val, const int32_t *cand_count,
+                                 void *stream) {
+    PFZ_REQUIRE(d_pad >= 8 && d_pad % 8 == 0 && cap >= 1, "pfz_dense_topn_exact_rescore: d_pad=%d, cap=%d", d_pad, cap);
+    if (n_rows <= 0) return 0;
+    CandRescoreParams P;
+    P.x = x_f64; P.y = y_f64; P.n_rows = n_rows; P.d_pad = d_pad; P.cap = cap; P.to_base = to_index_base;
+    P.row_map = row_map; P.cand_idx = cand_idx; P.cand_val = cand_val; P.count = cand_count;
+    const long long warps = (long long)n_rows * ((cap + 31) / 32);
+    const int grid = (int)(warps < (long long)SM_COUNT * 16 * 8 ? (warps + 7) / 8 : SM_COUNT * 16);
+    topn_exact_rescore_kernel<<<grid, 256, 0, as_stream(stream)>>>(P);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
+int pfz_dense_topn_select(const int32_t *cand_idx, const double *cand_val, const int32_t *cand_count, int32_t n_rows, int32_t cap, int32_t k,
+                          double min_similarity, int32_t self_match, int64_t from_index_base, const int32_t *row_map, int32_t *top_idx,
+                          double *top_val, void *stream) {
+    PFZ_REQUIRE(k >= 1 && cap >= 1, "pfz_dense_topn_select: k=%d, cap=%d must be >= 1", k, cap);
+    SelectParams P = {};
+    P.idx = cand_idx; P.val = cand_val; P.count = cand_count; P.n_rows = n_rows; P.n_cand = cap;
+    P.row_stride = cap; P.seg_len = cap; P.seg_stride = 0; P.row_map = row_map;
+    P.k = k; P.thr = min_similarity; P.self_match = self_match; P.from_base = from_index_base; P.top_idx = top_idx; P.top_val = top_val;
+    return topn_select_launch(P, as_stream(stream));
 }
 
 int pfz_dense_exact_rescore(const double *x_f64, const double *y_f64, int32_t n_from, int32_t n_to, int32_t d_pad, int32_t k, int32_t k_cand,

@@ -40,8 +40,11 @@ def dense_topk(x_bf16, y_bf16, k, min_similarity=0.0, self_match=False, from_ind
     n_from, d = x_bf16.shape
     n_to = y_bf16.shape[0]
     k = int(k)
-    if not 1 <= k <= 32:
-        raise NotImplementedError("dense top_n is limited to 32 per call")
+    if k < 1:
+        raise NotImplementedError("dense top_n must be >= 1")
+    if k > 32:
+        idx, val, _ = dense_topn_bounded(x_bf16, y_bf16, k, min_similarity, self_match, from_index_base, to_index_base, n_splits)
+        return idx, val
     if n_from == 0:
         return torch.empty((0, k), dtype=torch.int32, device=dev), torch.empty((0, k), dtype=torch.float64, device=dev)
     n_mblocks = (n_from + 127) // 128
@@ -160,10 +163,13 @@ def dense_topk_exact(xs, ys, k, min_similarity=0.0, self_match=False, from_index
     val float64[n_from,k], fallback row count int32[1] on the device); no host synchronisation."""
     dev = _dev()
     k = int(k)
-    if not 1 <= k <= 32:
-        raise NotImplementedError("dense top_n is limited to 32 per call")
+    if k < 1:
+        raise NotImplementedError("dense top_n must be >= 1")
     if xs.d_pad != ys.d_pad:
         raise ValueError(f"embedding widths differ: {xs.d_pad} vs {ys.d_pad} (padded)")
+    if k > 32:
+        idx, val, n_over = dense_topn_bounded(xs, ys, k, min_similarity, self_match, from_index_base, to_index_base, n_splits)
+        return idx, val, torch.full((1,), n_over, dtype=torch.int32, device=dev)
     if xs.n == 0:
         return (torch.empty((0, k), dtype=torch.int32, device=dev), torch.empty((0, k), dtype=torch.float64, device=dev),
                 torch.zeros(1, dtype=torch.int32, device=dev))
@@ -172,3 +178,108 @@ def dense_topk_exact(xs, ys, k, min_similarity=0.0, self_match=False, from_index
     idx, val, fb_rows, fb_count = exact_rescore(xs, ys, ci, cv, k, min_similarity, self_match, from_index_base, to_index_base)
     exact_fallback(xs, ys, idx, val, fb_rows, fb_count, min_similarity, self_match, from_index_base, to_index_base)
     return idx, val, fb_count
+
+
+# ---- top_n > 32, both precisions (DESIGN.md 4.7): bound, threshold pass, select -----------------------------------------------
+
+TOPN_WS_BYTES = 512 << 20          # bound lists + candidate buffers of one chunk of from-rows
+TOPN_LIST = 16                     # the bound pass runs the KMAX = 16 instantiation
+
+
+def topn_cap_for(k):
+    """Default candidate slots per row of the threshold pass: 4k rounded up to 32, at least 256."""
+    return max(256, (4 * int(k) + 31) // 32 * 32)
+
+
+def _splits(rows, n_ntiles):
+    mb = (rows + 127) // 128
+    return max(1, min(n_ntiles, (2 * SM_COUNT + mb - 1) // mb))
+
+
+def dense_topn_bounded(x, y, k, min_similarity=0.0, self_match=False, from_index_base=0, to_index_base=0, n_splits=None,
+                       cap=None, chunk_rows=None, events=None):
+    """Top-k of any size k (DESIGN.md 4.7); dense_topk and dense_topk_exact take this path for k > 32, and for k <= 32 it returns
+    what they return.  x, y: bf16 rows (to_bf16_rows) or ExactRows (stage_exact: the exact mode).
+
+    Per chunk of from-rows: a bound pass (the top-16 kernel with >= 2k/16 unmerged splits, then pfz_dense_topn_bound), the
+    threshold pass (pfz_dense_cos_cand[_f16], `cap` slots per row), in the exact mode the canonical re-score, and the select.
+    Rows with more than `cap` candidates are then re-run with the exact capacity; that takes one device-to-host read (their
+    number and the largest count).  Returns (idx int32[n_from,k], val float64[n_from,k], overflow row count).
+    `events` (a list) receives (stage name, CUDA event) pairs at the stage boundaries."""
+    dev = _dev()
+    k = int(k)
+    if k < 1:
+        raise NotImplementedError("dense top_n must be >= 1")
+    exact = isinstance(x, ExactRows)
+    xop, yop = (x.f16, y.f16) if exact else (x, y)
+    n_from, d = xop.shape
+    n_to = yop.shape[0]
+    idx = torch.empty((n_from, k), dtype=torch.int32, device=dev)
+    val = torch.empty((n_from, k), dtype=torch.float64, device=dev)
+    if n_from == 0:
+        return idx, val, 0
+    thr = float(min_similarity)
+    sel_thr = thr if exact else float(np.float32(thr))   # the bf16 kernel compares fp32 scores with float(min_similarity)
+    st = _stream()
+    n_ntiles = (n_to + 127) // 128
+    s_min = -(-2 * k // TOPN_LIST)
+    cap = max(1, min(n_to, int(cap) if cap else topn_cap_for(k)))
+    if chunk_rows is None:
+        per_row = 12 * (min(n_ntiles, max(s_min, 4)) * TOPN_LIST + cap) + 16
+        chunk_rows = max(128, TOPN_WS_BYTES // per_row // 128 * 128)
+    chunk_rows = max(1, int(chunk_rows))
+    topk_fn = "pfz_dense_cos_topk_f16" if exact else "pfz_dense_cos_topk"
+    cand_fn = "pfz_dense_cos_cand_f16" if exact else "pfz_dense_cos_cand"
+
+    def mark(name):
+        if events is not None:
+            e = torch.cuda.Event(enable_timing=True); e.record(); events.append((name, e))
+
+    def run_rows(xg, row_map, out_lo, thr_rows, cnt_rows, c, timed=True):
+        """Threshold pass, exact re-score and select of the rows xg (output rows row_map, or out_lo + r)."""
+        m = xg.shape[0]
+        ci = torch.empty((m, c), dtype=torch.int32, device=dev)
+        cv = torch.empty((m, c), dtype=torch.float64, device=dev)
+        sp = max(1, min(n_ntiles, int(n_splits) if n_splits else _splits(m, n_ntiles)))
+        _lib.call(cand_fn, _p(xg), _p(yop), m, n_to, d, thr, _p(thr_rows), int(to_index_base), sp, c, _p(ci), _p(cv), _p(cnt_rows), st)
+        if timed:
+            mark("select")
+        if exact:
+            xf = x.f64 if row_map is not None else x.f64[out_lo:out_lo + m]
+            _lib.call("pfz_dense_topn_exact_rescore", _p(xf), _p(y.f64), m, d, _p(row_map), int(to_index_base), c, _p(ci), _p(cv),
+                      _p(cnt_rows), st)
+        oi = idx if row_map is not None else idx[out_lo:out_lo + m]
+        ov = val if row_map is not None else val[out_lo:out_lo + m]
+        fb = int(from_index_base) + (0 if row_map is not None else out_lo)
+        _lib.call("pfz_dense_topn_select", _p(ci), _p(cv), _p(cnt_rows), m, c, k, sel_thr, int(bool(self_match)), fb, _p(row_map),
+                  _p(oi), _p(ov), st)
+
+    row_thr = torch.empty(n_from, dtype=torch.float32, device=dev)
+    counts = torch.empty(n_from, dtype=torch.int32, device=dev)
+    for lo in range(0, n_from, chunk_rows):
+        hi = min(n_from, lo + chunk_rows)
+        rows = hi - lo
+        mark("bound")
+        s = max(1, min(n_ntiles, max(s_min, int(n_splits) if n_splits else _splits(rows, n_ntiles))))
+        li = torch.empty((s, rows, TOPN_LIST), dtype=torch.int32, device=dev)
+        lv = torch.empty((s, rows, TOPN_LIST), dtype=torch.float64, device=dev)
+        _lib.call(topk_fn, _p(xop[lo:hi]), _p(yop), rows, n_to, d, TOPN_LIST, thr, int(bool(self_match)), int(from_index_base) + lo,
+                  int(to_index_base), s, _p(li), _p(lv), st)
+        _lib.call("pfz_dense_topn_bound", _p(li), _p(lv), s, rows, TOPN_LIST, k, int(exact),
+                  _p(x.norm16[lo:hi] if exact else None), _p(x.err16[lo:hi] if exact else None), _p(y.maxima if exact else None), d,
+                  thr, _p(row_thr[lo:hi]), st)
+        del li, lv
+        mark("threshold")
+        run_rows(xop[lo:hi], None, lo, row_thr[lo:hi], counts[lo:hi], cap)
+    mark("overflow")
+    over = counts > cap
+    n_over, max_cnt = torch.stack([over.sum(), counts.max().long()]).tolist()   # the one device-to-host read
+    if n_over:
+        rows_over = torch.argsort(over.int(), descending=True, stable=True)[:n_over].int()
+        chunk2 = max(1, TOPN_WS_BYTES // (12 * max_cnt))
+        for a in range(0, n_over, chunk2):
+            r = rows_over[a:a + chunk2]
+            cnt2 = torch.empty(len(r), dtype=torch.int32, device=dev)
+            run_rows(xop.index_select(0, r), r, 0, row_thr.index_select(0, r), cnt2, max_cnt, timed=False)
+    mark("end")
+    return idx, val, int(n_over)

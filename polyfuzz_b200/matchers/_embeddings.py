@@ -4,7 +4,9 @@ embedders themselves (`_embed`, Flair / SBERT / ...) are out of scope (SURVEY.md
 `embeddings_from` / `embeddings_to`, or an `embedding_method` callable `list[str] -> ndarray`.
 
 precision="bf16" (default) ranks bf16-rounded rows on fp32 tensor-core accumulators; precision="fp64" returns the canonical
-fp64 cosine top-n bit for bit (DESIGN.md 2 and 4.6), the reference's sklearn-branch scores up to the last bits."""
+fp64 cosine top-n bit for bit (DESIGN.md 2 and 4.6), the reference's sklearn-branch scores up to the last bits.  Any top_n
+works in both precisions: above 32 the rows take a bound pass, a threshold pass and a select on the GPU (DESIGN.md 4.7), with
+the same results as the top-k kernel would give; the only limit is memory for the n_from x top_n result."""
 from typing import Callable, List
 
 import numpy as np

@@ -41,6 +41,9 @@ for args, kw in (((fl, tl), dict(embeddings_from=ef, embeddings_to=et)), ((tl,),
     print(f"rank {rank} Embeddings lists={len(args)} identical={d.equals(s1)}", flush=True); ok = ok and d.equals(s1)
     d = Embeddings(min_similarity=0.0, top_n=5, distributed=True, precision="fp64").match(*args, **kw); s1 = Embeddings(min_similarity=0.0, top_n=5, precision="fp64").match(*args, **kw)
     print(f"rank {rank} Embeddings fp64 lists={len(args)} identical={d.equals(s1)}", flush=True); ok = ok and d.equals(s1)
+    # top_n > 32 on each shard (DESIGN.md 4.7), merged by merge_topk_any; like this whole script it needs two GPUs
+    d = Embeddings(min_similarity=0.0, top_n=50, distributed=True, precision="fp64").match(*args, **kw); s1 = Embeddings(min_similarity=0.0, top_n=50, precision="fp64").match(*args, **kw)
+    print(f"rank {rank} Embeddings fp64 top_n=50 lists={len(args)} identical={d.equals(s1)}", flush=True); ok = ok and d.equals(s1)
 flag = torch.tensor([int(ok)], device="cuda"); dist.all_reduce(flag, op=dist.ReduceOp.MIN)
 if rank == 0:
     print("DIST_CHECK", "PASS" if int(flag.item()) == 1 else "FAIL", flush=True)
