@@ -244,6 +244,18 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits,
                   int32_t n_from, int32_t *best_idx, double *best_score, int32_t *best_dist, void *stream);
 
+/* top-k sibling of pfz_lev_argbest: the k best to-strings per from-string (1 <= k <= 32), same candidates (score >= score_cutoff,
+ * to-row == from-row + self_shift excluded when exclude_self) and key (score desc, to-index asc).
+ * Replaces: rapidfuzz process.extract(query, to_list, scorer, limit=k), and the sort of the scorer values of
+ *           polyfuzz/models/_distance.py:98-99 where the reference takes np.argmax.
+ *   metric: NORM_LEV, RATIO, JARO or JARO_WINKLER; there is no distance output and no matrix.
+ *   part_idx / part_score: [n_splits][n_from][k] sorted lists, empty slots (-1, 0.0); merge them with pfz_topk_merge.   */
+int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                 int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
+                 const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
+                 int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
+                 int32_t k, int32_t *part_idx, double *part_score, int32_t *counter, void *stream);
+
 /* K3b  rapidfuzz's token / partial / weighted scorers with a fused per-row arg-best (csrc/pfz_fuzz.cu).
  * Replaces: process.extractOne(query, to_list, scorer=fuzz.WRatio | partial_ratio | token_*_ratio | ..., score_cutoff) at
  *           polyfuzz/models/_rapidfuzz.py:48,106-108 and the scorer loop of polyfuzz/models/_distance.py:98.
@@ -259,6 +271,15 @@ int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32
  * Best = first to-string (lowest index) with the maximal score >= score_cutoff; merge the splits with pfz_lev_merge.          */
 int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
                      int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream);
+
+/* top-k sibling of pfz_fuzz_argbest: the k best to-strings per from-string (1 <= k <= 32) under the same candidates and key.
+ * Replaces: rapidfuzz process.extract(query, to_list, scorer=..., score_cutoff=..., limit=k), and the sort of the scorer values
+ *           of polyfuzz/models/_distance.py:98-99 where the reference takes np.argmax.
+ * ptrs: as pfz_fuzz_argbest, except part_idx int32 / part_score float64 are [n_splits][n_from][k] sorted lists with empty slots
+ *       (-1, 0.0); merge them with pfz_topk_merge.                                                                               */
+int pfz_fuzz_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
+                  int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k,
+                  void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K4  dense cosine top-k for pre-computed embeddings (bf16 wgmma GEMM fed by TMA, top-k fused into the

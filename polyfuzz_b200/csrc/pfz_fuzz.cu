@@ -46,6 +46,7 @@ struct FuzzParams {
     const uint32_t *tok_blob; const int64_t *tok_off;       // token texts (code points) by token id
     int scorer; double cutoff; int exclude_self; int64_t self_shift;
     int n_splits; int32_t *part_idx; double *part_score; int n_from; int32_t *counter;
+    int k;                                                  // top-k epilogue: list length; part_* are [n_splits][n_from][k]
 };
 
 // ---- scalar scorer algebra (double, no contraction) -- mirrors oracle/fuzz.py line by line -------------------------------------
@@ -210,8 +211,11 @@ __device__ int fz_diff_indel(const int32_t *a, int na, const int32_t *b, int nb,
     return la + lb - 2 * (int)row[lb];
 }
 
-template <int NW, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) fuzz_kernel(const FuzzParams P) {
+// TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings
+// (the group's body is a do/while(0), so a lane that skips its pair still reaches the warp-wide offer).
+// (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; 0 = unspecified)
+template <int NW, int WARPS, bool TOPK = false>
+__global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const FuzzParams P) {
     extern __shared__ __align__(16) unsigned char dyn[];
     const int lane = lane_id();
     const int w = threadIdx.x >> 5;
@@ -255,115 +259,127 @@ __global__ void __launch_bounds__(WARPS * 32) fuzz_kernel(const FuzzParams P) {
         const uint64_t *peq0 = peq_all, *peq1 = peq_all + 256 * NW, *peq2 = peq_all + 2 * 256 * NW;
 
         double best_s = 0.0; int best_j = -1;
+        WarpTopK top;
+        if constexpr (TOPK) top.init(P.k);
         for (int g = g_lo; g < g_hi; ++g) {
-            const int p = g * 32 + lane;
-            if (p >= P.n_to) continue;
-            const int orig = P.sorig[p];
-            if (P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) continue;
-            TextRef t0{P.packed[0] + P.grp_off[0][g] + lane, P.slen[0][p]};
-            TextRef t1{P.packed[1] + P.grp_off[1][g] + lane, P.slen[1][p]};
-            TextRef t2{P.packed[2] + P.grp_off[2][g] + lane, P.slen[2][p]};
-            const int lb = t0.n;
-            const double cut = P.cutoff;
-            // token-set facts of the pair, computed on demand
-            bool tok_done = false; TokInfo ti{0, 0, 0, 0, 0, 0};
-            const int32_t *btok = P.T.tok_ids + P.T.tok_ptr[orig];
-            const int nb = P.T.tok_ptr[orig + 1] - P.T.tok_ptr[orig];
-            const int nb_all = P.T.n_tok_all[orig];
-            auto tok = [&]() {
-                if (!tok_done) {
-                    if ((asig & P.T.sig[orig]) == 0ull) {   // no common token possible: differences are the whole distinct-token strings
-                        ti.n_common = 0; ti.sect_len = 0; ti.ab_len = lau; ti.ba_len = t2.n; ti.n_ab = na; ti.n_ba = nb;
-                    } else ti = fz_tok_info(atok, na, btok, nb, P.tok_off);
-                    tok_done = true;
-                }
-            };
-            auto token_sort = [&](double c) { return fz_ratio(fz_lcs<NW>(peq1, las, t1), las, t1.n, c); };
-            auto token_set = [&](double c) -> double {
-                if (c > 100.0) return 0.0;
-                if (na == 0 || nb == 0) return 0.0;
-                tok();
-                if (ti.n_common && (ti.n_ab == 0 || ti.n_ba == 0)) return 100.0;
-                const int sect_len = ti.sect_len;
-                const int sect_ab_len = sect_len + (sect_len != 0) + ti.ab_len;
-                const int sect_ba_len = sect_len + (sect_len != 0) + ti.ba_len;
-                double result = 0.0;
-                const double cd = ceil(__dmul_rn((double)(sect_ab_len + sect_ba_len), __dsub_rn(1.0, __ddiv_rn(c, 100.0))));
-                const int dist = ti.n_common == 0 ? (lau + t2.n - 2 * fz_lcs<NW>(peq2, lau, t2))
-                                                  : fz_diff_indel(atok, na, btok, nb, P.tok_blob, P.tok_off);
-                if ((double)dist <= cd) result = fz_norm_distance(dist, sect_ab_len + sect_ba_len, c);
-                if (!sect_len) return result;
-                const double r_ab = fz_norm_distance((sect_len != 0) + ti.ab_len, sect_len + sect_ab_len, c);
-                const double r_ba = fz_norm_distance((sect_len != 0) + ti.ba_len, sect_len + sect_ba_len, c);
-                return fmax(result, fmax(r_ab, r_ba));
-            };
-            auto partial = [&](const uint64_t *peq, int m, const TextRef &t, double c) {
-                return fz_partial_from_best(fz_partial_best<NW>(peq, m, t), m == 0 && t.n == 0, c);
-            };
-            auto partial_token_ratio = [&](double c) -> double {
-                tok();
-                if (ti.n_common) return 100.0;
-                const double result = partial(peq1, las, t1, c);
-                if (na_all == na && nb_all == nb) return result;
-                c = fmax(c, result);
-                return fmax(result, partial(peq2, lau, t2, c));
-            };
-
-            double sc = 0.0;
-            switch (sc_id) {
-                case FZ_RATIO: sc = fz_ratio(fz_lcs<NW>(peq0, la, t0), la, lb, cut); break;
-                case FZ_QRATIO: sc = (la == 0 || lb == 0) ? 0.0 : fz_ratio(fz_lcs<NW>(peq0, la, t0), la, lb, cut); break;
-                case FZ_PARTIAL: sc = partial(peq0, la, t0, cut); break;
-                case FZ_TSORT: sc = token_sort(cut); break;
-                case FZ_TSET: sc = token_set(cut); break;
-                case FZ_TRATIO: sc = fmax(token_set(cut), token_sort(cut)); break;
-                case FZ_PTSORT: sc = partial(peq1, las, t1, cut); break;
-                case FZ_PTSET: {
-                    if (na == 0 || nb == 0) { sc = 0.0; break; }
+            double cand_s = 0.0; int cand_j = -1;
+            do {
+                const int p = g * 32 + lane;
+                if (p >= P.n_to) continue;
+                const int orig = P.sorig[p];
+                if (P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) continue;
+                TextRef t0{P.packed[0] + P.grp_off[0][g] + lane, P.slen[0][p]};
+                TextRef t1{P.packed[1] + P.grp_off[1][g] + lane, P.slen[1][p]};
+                TextRef t2{P.packed[2] + P.grp_off[2][g] + lane, P.slen[2][p]};
+                const int lb = t0.n;
+                const double cut = P.cutoff;
+                // token-set facts of the pair, computed on demand
+                bool tok_done = false; TokInfo ti{0, 0, 0, 0, 0, 0};
+                const int32_t *btok = P.T.tok_ids + P.T.tok_ptr[orig];
+                const int nb = P.T.tok_ptr[orig + 1] - P.T.tok_ptr[orig];
+                const int nb_all = P.T.n_tok_all[orig];
+                auto tok = [&]() {
+                    if (!tok_done) {
+                        if ((asig & P.T.sig[orig]) == 0ull) {   // no common token possible: differences are the whole distinct-token strings
+                            ti.n_common = 0; ti.sect_len = 0; ti.ab_len = lau; ti.ba_len = t2.n; ti.n_ab = na; ti.n_ba = nb;
+                        } else ti = fz_tok_info(atok, na, btok, nb, P.tok_off);
+                        tok_done = true;
+                    }
+                };
+                auto token_sort = [&](double c) { return fz_ratio(fz_lcs<NW>(peq1, las, t1), las, t1.n, c); };
+                auto token_set = [&](double c) -> double {
+                    if (c > 100.0) return 0.0;
+                    if (na == 0 || nb == 0) return 0.0;
                     tok();
-                    sc = ti.n_common ? 100.0 : partial(peq2, lau, t2, cut);
-                    break;
-                }
-                case FZ_PTRATIO: sc = partial_token_ratio(cut); break;
-                default: {                                  // WRatio
-                    if (la == 0 || lb == 0) { sc = 0.0; break; }
-                    const double len_ratio = la > lb ? __ddiv_rn((double)la, (double)lb) : __ddiv_rn((double)lb, (double)la);
-                    double end_ratio = fz_ratio(fz_lcs<NW>(peq0, la, t0), la, lb, cut);
-                    double c = cut;
-                    if (len_ratio < 1.5) {
-                        c = __ddiv_rn(fmax(c, end_ratio), 0.95);
-                        sc = fmax(end_ratio, __dmul_rn(fmax(token_set(c), token_sort(c)), 0.95));
+                    if (ti.n_common && (ti.n_ab == 0 || ti.n_ba == 0)) return 100.0;
+                    const int sect_len = ti.sect_len;
+                    const int sect_ab_len = sect_len + (sect_len != 0) + ti.ab_len;
+                    const int sect_ba_len = sect_len + (sect_len != 0) + ti.ba_len;
+                    double result = 0.0;
+                    const double cd = ceil(__dmul_rn((double)(sect_ab_len + sect_ba_len), __dsub_rn(1.0, __ddiv_rn(c, 100.0))));
+                    const int dist = ti.n_common == 0 ? (lau + t2.n - 2 * fz_lcs<NW>(peq2, lau, t2))
+                                                      : fz_diff_indel(atok, na, btok, nb, P.tok_blob, P.tok_off);
+                    if ((double)dist <= cd) result = fz_norm_distance(dist, sect_ab_len + sect_ba_len, c);
+                    if (!sect_len) return result;
+                    const double r_ab = fz_norm_distance((sect_len != 0) + ti.ab_len, sect_len + sect_ab_len, c);
+                    const double r_ba = fz_norm_distance((sect_len != 0) + ti.ba_len, sect_len + sect_ba_len, c);
+                    return fmax(result, fmax(r_ab, r_ba));
+                };
+                auto partial = [&](const uint64_t *peq, int m, const TextRef &t, double c) {
+                    return fz_partial_from_best(fz_partial_best<NW>(peq, m, t), m == 0 && t.n == 0, c);
+                };
+                auto partial_token_ratio = [&](double c) -> double {
+                    tok();
+                    if (ti.n_common) return 100.0;
+                    const double result = partial(peq1, las, t1, c);
+                    if (na_all == na && nb_all == nb) return result;
+                    c = fmax(c, result);
+                    return fmax(result, partial(peq2, lau, t2, c));
+                };
+
+                double sc = 0.0;
+                switch (sc_id) {
+                    case FZ_RATIO: sc = fz_ratio(fz_lcs<NW>(peq0, la, t0), la, lb, cut); break;
+                    case FZ_QRATIO: sc = (la == 0 || lb == 0) ? 0.0 : fz_ratio(fz_lcs<NW>(peq0, la, t0), la, lb, cut); break;
+                    case FZ_PARTIAL: sc = partial(peq0, la, t0, cut); break;
+                    case FZ_TSORT: sc = token_sort(cut); break;
+                    case FZ_TSET: sc = token_set(cut); break;
+                    case FZ_TRATIO: sc = fmax(token_set(cut), token_sort(cut)); break;
+                    case FZ_PTSORT: sc = partial(peq1, las, t1, cut); break;
+                    case FZ_PTSET: {
+                        if (na == 0 || nb == 0) { sc = 0.0; break; }
+                        tok();
+                        sc = ti.n_common ? 100.0 : partial(peq2, lau, t2, cut);
                         break;
                     }
-                    const double ps = len_ratio <= 8.0 ? 0.9 : 0.6;
-                    c = __ddiv_rn(fmax(c, end_ratio), ps);
-                    end_ratio = fmax(end_ratio, __dmul_rn(partial(peq0, la, t0, c), ps));
-                    c = __ddiv_rn(fmax(c, end_ratio), 0.95);
-                    sc = fmax(end_ratio, __dmul_rn(__dmul_rn(partial_token_ratio(c), 0.95), ps));
+                    case FZ_PTRATIO: sc = partial_token_ratio(cut); break;
+                    default: {                                  // WRatio
+                        if (la == 0 || lb == 0) { sc = 0.0; break; }
+                        const double len_ratio = la > lb ? __ddiv_rn((double)la, (double)lb) : __ddiv_rn((double)lb, (double)la);
+                        double end_ratio = fz_ratio(fz_lcs<NW>(peq0, la, t0), la, lb, cut);
+                        double c = cut;
+                        if (len_ratio < 1.5) {
+                            c = __ddiv_rn(fmax(c, end_ratio), 0.95);
+                            sc = fmax(end_ratio, __dmul_rn(fmax(token_set(c), token_sort(c)), 0.95));
+                            break;
+                        }
+                        const double ps = len_ratio <= 8.0 ? 0.9 : 0.6;
+                        c = __ddiv_rn(fmax(c, end_ratio), ps);
+                        end_ratio = fmax(end_ratio, __dmul_rn(partial(peq0, la, t0, c), ps));
+                        c = __ddiv_rn(fmax(c, end_ratio), 0.95);
+                        sc = fmax(end_ratio, __dmul_rn(__dmul_rn(partial_token_ratio(c), 0.95), ps));
+                    }
                 }
-            }
-            if (sc >= P.cutoff && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; }
+                if constexpr (TOPK) { if (sc >= P.cutoff) { cand_s = sc; cand_j = orig; } }
+                else if (sc >= P.cutoff && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; }
+            } while (0);
+            if constexpr (TOPK) top.offer(cand_s, cand_j);
         }
-        // first maximal score = lowest original index among the maxima
+        if constexpr (TOPK) {
+            const size_t o = ((size_t)split * P.n_from + i) * P.k;
+            top.store(P.part_idx + o, P.part_score + o);
+        } else {
+            // first maximal score = lowest original index among the maxima
 #pragma unroll
-        for (int d = 16; d; d >>= 1) {
-            const double os = shfl_d(best_s, lane ^ d);
-            const int oj = __shfl_xor_sync(FULL, best_j, d);
-            if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; }
-        }
-        if (lane == 0) {
-            const size_t o = (size_t)split * P.n_from + i;
-            P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0;
+            for (int d = 16; d; d >>= 1) {
+                const double os = shfl_d(best_s, lane ^ d);
+                const int oj = __shfl_xor_sync(FULL, best_j, d);
+                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; }
+            }
+            if (lane == 0) {
+                const size_t o = (size_t)split * P.n_from + i;
+                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0;
+            }
         }
         __syncwarp();
     }
 }
 
-template <int NW>
+template <int NW, bool TOPK>
 static int launch_fuzz(const FuzzParams &P, int sms, cudaStream_t st) {
     constexpr int WARPS = NW == 1 ? 4 : NW == 2 ? 2 : 1;
     const size_t smem = (size_t)WARPS * 3 * 256 * NW * 8;
-    auto kernel = fuzz_kernel<NW, WARPS>;
+    auto kernel = fuzz_kernel<NW, WARPS, TOPK>;
     PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
@@ -377,20 +393,10 @@ static int launch_fuzz(const FuzzParams &P, int sms, cudaStream_t st) {
     return 0;
 }
 
-}  // namespace pfz
-
-using namespace pfz;
-
-extern "C" {
-
-/* ptrs: 38 device pointers in the order of PfzFuzzArgs below (one flat array keeps the C ABI free of structs) */
-int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
-                     double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream) {
-    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_argbest: expected 38 pointers, got %d", n_ptrs);
-    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_argbest: unknown scorer %d", scorer);
-    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4, "pfz_fuzz_argbest: n_words %d unsupported (1, 2, 4: strings up to 255 code points)", n_words);
-    PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_argbest: n_splits < 1");
-    if (n_ids <= 0 || n_to <= 0) return 0;
+// the 38 pointers of the C ABI (order: include/pfz.h) -> FuzzParams; part_idx / part_score as the caller's entry point lays them out
+template <bool TOPK>
+static int run_fuzz(const void *const *ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
+                    double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k_out, void *stream) {
     cudaStream_t st = as_stream(stream);
     int dev = 0, sms = 0;
     PFZ_CUDA_OK(cudaGetDevice(&dev));
@@ -409,10 +415,39 @@ int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, in
     P.part_idx = (int32_t *)ptrs[k++]; P.part_score = (double *)ptrs[k++]; P.counter = (int32_t *)ptrs[k++];                  // 37
     k++;                                                                            // 38: reserved
     P.n_ids = n_ids; P.n_to = n_to; P.scorer = scorer; P.cutoff = score_cutoff; P.exclude_self = exclude_self; P.self_shift = self_shift;
-    P.n_splits = n_splits; P.n_from = n_from;
+    P.n_splits = n_splits; P.n_from = n_from; P.k = k_out;
     PFZ_CUDA_OK(cudaMemsetAsync(P.counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
-    if (n_words == 1) return launch_fuzz<1>(P, sms, st);
-    if (n_words == 2) return launch_fuzz<2>(P, sms, st);
-    return launch_fuzz<4>(P, sms, st);
+    if (n_words == 1) return launch_fuzz<1, TOPK>(P, sms, st);
+    if (n_words == 2) return launch_fuzz<2, TOPK>(P, sms, st);
+    return launch_fuzz<4, TOPK>(P, sms, st);
+}
+
+}  // namespace pfz
+
+using namespace pfz;
+
+extern "C" {
+
+/* ptrs: 38 device pointers in the order of PfzFuzzArgs below (one flat array keeps the C ABI free of structs) */
+int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
+                     double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream) {
+    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_argbest: expected 38 pointers, got %d", n_ptrs);
+    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_argbest: unknown scorer %d", scorer);
+    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4, "pfz_fuzz_argbest: n_words %d unsupported (1, 2, 4: strings up to 255 code points)", n_words);
+    PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_argbest: n_splits < 1");
+    if (n_ids <= 0 || n_to <= 0) return 0;
+    return run_fuzz<false>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, n_splits, 1, stream);
+}
+
+/* ptrs: as pfz_fuzz_argbest, with part_idx / part_score laid out [n_splits][n_from][k] */
+int pfz_fuzz_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
+                  double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k, void *stream) {
+    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_topk: expected 38 pointers, got %d", n_ptrs);
+    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_topk: unknown scorer %d", scorer);
+    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4, "pfz_fuzz_topk: n_words %d unsupported (1, 2, 4: strings up to 255 code points)", n_words);
+    PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_topk: n_splits < 1");
+    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_fuzz_topk: k=%d unsupported (1..32)", k);
+    if (n_ids <= 0 || n_to <= 0) return 0;
+    return run_fuzz<true>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, n_splits, k, stream);
 }
 }

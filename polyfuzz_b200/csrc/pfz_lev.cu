@@ -62,6 +62,7 @@ struct LevParams {
     int32_t *part_idx; double *part_score; int32_t *part_dist;     // [n_splits][n_from]
     int32_t *matrix; int64_t matrix_ld;                           // optional full matrix [n_from][n_to]
     int n_from; int32_t *counter;
+    int k;                              // top-k epilogue: list length; part_idx / part_score are [n_splits][n_from][k]
 };
 
 __device__ __forceinline__ double score_of(int metric, int d, int la, int lb) {
@@ -76,8 +77,10 @@ template <> struct WordOps<uint64_t> { static constexpr int BITS = 64; static __
 
 // One warp scores pattern `pat` against every to-string of its split.  LCS = false: Levenshtein (Myers 1999,
 // blocks: Hyyro 2003); LCS = true: longest common subsequence (Hyyro 2004) -> Indel = la + lb - 2*LCS.
-template <typename W, int NW, bool LCS, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) lev_kernel(const LevParams P) {
+// TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings.
+// (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; 0 = unspecified)
+template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false>
+__global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const LevParams P) {
     constexpr int B = WordOps<W>::BITS;
     extern __shared__ __align__(16) unsigned char dyn[];
     const int lane = lane_id();
@@ -113,7 +116,10 @@ __global__ void __launch_bounds__(WARPS * 32) lev_kernel(const LevParams P) {
         const int last_blk = m > 0 ? (m - 1) / B : 0;
 
         double best_s = 0.0; int best_j = -1, best_d = -1;
+        WarpTopK top;
+        if constexpr (TOPK) top.init(P.k);
         for (int g = g_lo; g < g_hi; ++g) {
+            double cand_s = 0.0; int cand_j = -1;
             const int p = g * 32 + lane;
             const bool have = p < P.n_to;
             const int n = have ? P.slen[p] : 0;
@@ -204,19 +210,26 @@ __global__ void __launch_bounds__(WARPS * 32) lev_kernel(const LevParams P) {
                 const double sc = score_of(P.metric, dist, m, n);
                 bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift);
                 if ((P.metric == PFZ_METRIC_NORM_LEV || P.metric == PFZ_METRIC_RATIO) && !(sc >= P.cutoff)) ok = false;
-                if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = dist; }
+                if constexpr (TOPK) { cand_s = sc; cand_j = ok ? orig : -1; }
+                else if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = dist; }
             }
+            if constexpr (TOPK) top.offer(cand_s, cand_j);
         }
-        // first maximal score = lowest original index among the maxima
+        if constexpr (TOPK) {
+            const size_t o = ((size_t)split * P.n_from + i) * P.k;
+            top.store(P.part_idx + o, P.part_score + o);
+        } else {
+            // first maximal score = lowest original index among the maxima
 #pragma unroll
-        for (int d = 16; d; d >>= 1) {
-            const double os = shfl_d(best_s, lane ^ d);
-            const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
-            if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
-        }
-        if (lane == 0) {
-            const size_t o = (size_t)split * P.n_from + i;
-            P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
+            for (int d = 16; d; d >>= 1) {
+                const double os = shfl_d(best_s, lane ^ d);
+                const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
+                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
+            }
+            if (lane == 0) {
+                const size_t o = (size_t)split * P.n_from + i;
+                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
+            }
         }
         __syncwarp();
     }
@@ -241,7 +254,7 @@ template <typename W> __device__ __forceinline__ int low_bit(W x);
 template <> __device__ __forceinline__ int low_bit<uint32_t>(uint32_t x) { return __ffs(x) - 1; }
 template <> __device__ __forceinline__ int low_bit<uint64_t>(uint64_t x) { return __ffsll(x) - 1; }
 
-template <typename W, int NW, int WARPS>
+template <typename W, int NW, int WARPS, bool TOPK = false>
 __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
     constexpr int B = WordOps<W>::BITS;
     constexpr int STORE = B * NW;                                           // max matches per lane
@@ -279,7 +292,10 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
         const int last_blk = m > 0 ? (m - 1) / B : 0;                          // blocks above it hold no pattern bits
 
         double best_s = 0.0; int best_j = -1, best_d = -1;
+        WarpTopK top;
+        if constexpr (TOPK) top.init(P.k);
         for (int g = g_lo; g < g_hi; ++g) {
+            double cand_s = 0.0; int cand_j = -1;
             const int p = g * 32 + lane;
             const bool have = p < P.n_to;
             const int n = have ? P.slen[p] : 0;
@@ -346,18 +362,25 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
             }
             if (have) {
                 bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) && sc >= P.cutoff;
-                if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = k; }
+                if constexpr (TOPK) { cand_s = sc; cand_j = ok ? orig : -1; }
+                else if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = k; }
             }
+            if constexpr (TOPK) top.offer(cand_s, cand_j);
         }
+        if constexpr (TOPK) {
+            const size_t o = ((size_t)split * P.n_from + i) * P.k;
+            top.store(P.part_idx + o, P.part_score + o);
+        } else {
 #pragma unroll
-        for (int d = 16; d; d >>= 1) {
-            const double os = shfl_d(best_s, lane ^ d);
-            const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
-            if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
-        }
-        if (lane == 0) {
-            const size_t o = (size_t)split * P.n_from + i;
-            P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
+            for (int d = 16; d; d >>= 1) {
+                const double os = shfl_d(best_s, lane ^ d);
+                const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
+                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
+            }
+            if (lane == 0) {
+                const size_t o = (size_t)split * P.n_from + i;
+                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
+            }
         }
         __syncwarp();
     }
@@ -379,11 +402,11 @@ __global__ void lev_merge_kernel(const int32_t *__restrict__ part_idx, const dou
     }
 }
 
-template <typename W, int NW, bool LCS>
+template <typename W, int NW, bool LCS, bool TOPK>
 static int launch_lev(const LevParams &P, int sms, cudaStream_t st) {
     constexpr int WARPS = 4;
     const size_t smem = (size_t)WARPS * 256 * NW * sizeof(W);
-    auto kernel = lev_kernel<W, NW, LCS, WARPS>;
+    auto kernel = lev_kernel<W, NW, LCS, WARPS, TOPK>;
     PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
@@ -399,12 +422,12 @@ static int launch_lev(const LevParams &P, int sms, cudaStream_t st) {
 
 // Shared memory per warp: Peq (256 x NW words) plus the match store (32 lanes x B*NW bytes), the same size again.
 // Up to 64 KB per CTA: 4 warps up to 256 code points, 2 at 512, 1 at 1 024.
-template <typename W, int NW>
+template <typename W, int NW, bool TOPK>
 static int launch_jaro(const LevParams &P, int sms, cudaStream_t st) {
     constexpr size_t PER_WARP = 2 * 256 * NW * sizeof(W);
     constexpr int WARPS = PER_WARP * 4 <= 65536 ? 4 : PER_WARP * 2 <= 65536 ? 2 : 1;
     const size_t smem = (size_t)WARPS * PER_WARP;
-    auto kernel = jaro_kernel<W, NW, WARPS>;
+    auto kernel = jaro_kernel<W, NW, WARPS, TOPK>;
     PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
@@ -416,6 +439,33 @@ static int launch_jaro(const LevParams &P, int sms, cudaStream_t st) {
     kernel<<<dim3(gx, P.n_splits), WARPS * 32, smem, st>>>(P);
     PFZ_LAUNCH_OK();
     return 0;
+}
+
+// word class -> kernel instantiation (the metric picks Levenshtein, Indel or Jaro)
+template <bool TOPK>
+static int launch_class(const LevParams &P, int n_words, int sms, cudaStream_t st) {
+    if (P.metric == PFZ_METRIC_JARO || P.metric == PFZ_METRIC_JARO_WINKLER) {
+        switch (n_words) {
+            case 0: return launch_jaro<uint32_t, 1, TOPK>(P, sms, st);
+            case 1: return launch_jaro<uint64_t, 1, TOPK>(P, sms, st);
+            case 2: return launch_jaro<uint64_t, 2, TOPK>(P, sms, st);
+            case 4: return launch_jaro<uint64_t, 4, TOPK>(P, sms, st);
+            case 8: return launch_jaro<uint64_t, 8, TOPK>(P, sms, st);
+            default: return launch_jaro<uint64_t, 16, TOPK>(P, sms, st);
+        }
+    }
+    const bool lcs = (P.metric == PFZ_METRIC_INDEL || P.metric == PFZ_METRIC_RATIO);
+#define PFZ_LEV_CASE(NWv, Wt)                                                            \
+    return lcs ? launch_lev<Wt, NWv, true, TOPK>(P, sms, st) : launch_lev<Wt, NWv, false, TOPK>(P, sms, st)
+    switch (n_words) {
+        case 0: PFZ_LEV_CASE(1, uint32_t);
+        case 1: PFZ_LEV_CASE(1, uint64_t);
+        case 2: PFZ_LEV_CASE(2, uint64_t);
+        case 4: PFZ_LEV_CASE(4, uint64_t);
+        case 8: PFZ_LEV_CASE(8, uint64_t);
+        default: PFZ_LEV_CASE(16, uint64_t);
+    }
+#undef PFZ_LEV_CASE
 }
 
 }  // namespace pfz
@@ -452,29 +502,29 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
     PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
     LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
-                exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter};
-    if (jaro) {
-        switch (n_words) {
-            case 0: return launch_jaro<uint32_t, 1>(P, sms, st);
-            case 1: return launch_jaro<uint64_t, 1>(P, sms, st);
-            case 2: return launch_jaro<uint64_t, 2>(P, sms, st);
-            case 4: return launch_jaro<uint64_t, 4>(P, sms, st);
-            case 8: return launch_jaro<uint64_t, 8>(P, sms, st);
-            default: return launch_jaro<uint64_t, 16>(P, sms, st);
-        }
-    }
-    const bool lcs = (metric == PFZ_METRIC_INDEL || metric == PFZ_METRIC_RATIO);
-#define PFZ_LEV_CASE(NWv, Wt)                                                            \
-    return lcs ? launch_lev<Wt, NWv, true>(P, sms, st) : launch_lev<Wt, NWv, false>(P, sms, st)
-    switch (n_words) {
-        case 0: PFZ_LEV_CASE(1, uint32_t);
-        case 1: PFZ_LEV_CASE(1, uint64_t);
-        case 2: PFZ_LEV_CASE(2, uint64_t);
-        case 4: PFZ_LEV_CASE(4, uint64_t);
-        case 8: PFZ_LEV_CASE(8, uint64_t);
-        default: PFZ_LEV_CASE(16, uint64_t);
-    }
-#undef PFZ_LEV_CASE
+                exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter, 1};
+    return launch_class<false>(P, n_words, sms, st);
+}
+
+int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                 int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                 const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                 int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER,
+                "pfz_lev_topk: metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER)", metric);
+    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_lev_topk: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
+    PFZ_REQUIRE(n_splits >= 1, "pfz_lev_topk: n_splits < 1");
+    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_lev_topk: k=%d unsupported (1..32)", k);
+    if (n_ids <= 0 || n_to < 0) return 0;
+    cudaStream_t st = as_stream(stream);
+    int dev = 0, sms = 0;
+    PFZ_CUDA_OK(cudaGetDevice(&dev));
+    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
+    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
+                exclude_self, self_shift, n_splits, part_idx, part_score, nullptr, nullptr, 0, n_from, counter, k};
+    return launch_class<true>(P, n_words, sms, st);
 }
 
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits, int32_t n_from,

@@ -10,7 +10,8 @@ polyfuzz/models/_distance.py:89-102) and rapidfuzz's published definitions:
 The Jaro metrics are computed on code points, from-string first (the reference calls scorer(from_string, to_string),
 polyfuzz/models/_distance.py:98); their best_dist is the number of matching characters, and they have no distance
 matrix (want_matrix=True raises ValueError).
-Best match of a from-string = first to-string (lowest index) with the maximal score >= score_cutoff.
+Best match of a from-string = first to-string (lowest index) with the maximal score >= score_cutoff; the top-k functions
+return the k best under the same key (score desc, index asc), k <= 32.
 
 Two levels: `EditQueries` / `EditTargets` stage a from-list / to-list in HBM once (host packing, length sort,
 alphabet batches); `edit_argbest_staged` only enqueues kernels, so a staged pair can be scored repeatedly
@@ -20,7 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import _dev, _p, _stream, _to_dev
+from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
 METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3, "jaro": 4, "jaro_winkler": 5}
@@ -177,6 +178,55 @@ def edit_argbest(from_list, to_list, metric="ratio", score_cutoff=0.0, exclude_s
     Q = EditQueries(from_list)
     T = EditTargets(to_list)
     return edit_argbest_staged(Q, T, metric, score_cutoff, exclude_self, self_shift, want_matrix, n_splits)
+
+
+TOPK_MAX = 32
+TOPK_METRICS = ("norm_lev", "ratio", "jaro", "jaro_winkler")
+
+
+def check_top_n(k):
+    """top_n of the edit-distance matchers: an int in 1..32 (the k best of a row are held in one warp's registers)."""
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= TOPK_MAX:
+        raise ValueError(f"top_n must be an int from 1 to {TOPK_MAX}, got {k!r}")
+    return int(k)
+
+
+def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, to_index_base=0):
+    """Kernels only: the k best to-strings per from-string (pfz_lev_topk, then pfz_topk_merge over the to-splits), with the
+    candidates and the key of edit_argbest_staged.  Returns device (idx int32[n_from, k] (-1 = empty slot; + to_index_base
+    otherwise), score float64[n_from, k] (0.0 in empty slots))."""
+    k = check_top_n(k)
+    if metric not in TOPK_METRICS:
+        raise ValueError(f"top-k is available for the metrics {TOPK_METRICS}, not {metric!r}")
+    dev = _dev()
+    n_from, n_to = Q.n, T.n
+    if n_from == 0 or n_to == 0:
+        return (torch.full((n_from, k), -1, dtype=torch.int32, device=dev), torch.zeros((n_from, k), dtype=torch.float64, device=dev))
+    if n_splits is None:
+        n_splits = default_splits(n_from, T.n_grp)
+    n_splits = max(1, min(int(n_splits), T.n_grp))
+    part_idx = torch.full((n_splits, n_from, k), -1, dtype=torch.int32, device=dev)
+    part_score = torch.zeros((n_splits, n_from, k), dtype=torch.float64, device=dev)
+    counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
+    for d_table, groups in Q.batches:
+        _lib.call("pfz_lev_pack", _p(T.d_blob), _p(T.d_off), _p(T.d_order), n_to, _p(d_table), _p(T.d_goff), _p(T.packed), _p(T.slen), _stream())
+        for nw, d_ids, n_ids in groups:
+            _lib.call("pfz_lev_topk", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
+                      _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)), int(self_shift),
+                      n_splits, k, _p(part_idx), _p(part_score), _p(counter), _stream())
+    idx, score = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
+    if to_index_base:
+        idx = torch.where(idx >= 0, idx + int(to_index_base), idx)
+    return idx, score
+
+
+def edit_topk(from_list, to_list, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None):
+    """Host lists in, device tensors out (see edit_topk_staged)."""
+    k = check_top_n(k)
+    _dev()
+    Q = EditQueries(from_list)
+    T = EditTargets(to_list)
+    return edit_topk_staged(Q, T, k, metric, score_cutoff, exclude_self, self_shift, n_splits)
 
 
 def lev_merge(part_idx, part_score, part_dist):

@@ -14,8 +14,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .editdist import N_CODE_POINTS, _alphabet_batches, _blob_to_dev, default_splits
-from .engine import _dev, _p, _stream, _to_dev
+from .editdist import N_CODE_POINTS, _alphabet_batches, _blob_to_dev, check_top_n, default_splits
+from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
 SCORER = {"ratio": 0, "QRatio": 1, "partial_ratio": 2, "token_sort_ratio": 3, "token_set_ratio": 4, "token_ratio": 5,
@@ -64,19 +64,13 @@ class _Side:
         return out + [self.d_tok_ptr, self.d_tok_ids, self.d_sig, self.d_n_all]
 
 
-def fuzz_argbest(from_list, to_list, scorer="WRatio", score_cutoff=0.0, exclude_self=False, n_splits=None, self_shift=0,
-                 to_index_base=0):
-    """Best to-string per from-string under a rapidfuzz scorer (scores in [0, 100]).  Returns device tensors
-    (best_idx int32[n_from] (-1: no to-string reached score_cutoff), best_score float64[n_from]).
-    exclude_self skips to-row == from-row + self_shift; to_index_base is added to the returned indices (row-block shards)."""
-    if scorer not in SCORER:
-        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
+def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift, to_index_base, k):
+    """Stage both lists (tokens, one vocabulary, the three to-side layouts, one symbol table per alphabet batch) and enqueue
+    K3b for every batch and word class: pfz_fuzz_argbest with part_* [n_splits, n_from] when k is None, else pfz_fuzz_topk
+    with part_* [n_splits, n_from, k].  Returns (part_idx, part_score, n_splits, staged): `staged` keeps the staged buffers
+    alive until the caller has synchronised."""
     dev = _dev()
     n_from, n_to = len(from_list), len(to_list)
-    best_idx = torch.full((max(n_from, 1),), -1, dtype=torch.int32, device=dev)
-    best_score = torch.zeros(max(n_from, 1), dtype=torch.float64, device=dev)
-    if n_from == 0 or n_to == 0:
-        return best_idx[:n_from], best_score[:n_from]
     same = to_list is from_list and not to_index_base
     ftoks, fS, fU = _derive(from_list)
     ttoks, tS, tU = (ftoks, fS, fU) if same else _derive(to_list)
@@ -106,9 +100,9 @@ def fuzz_argbest(from_list, to_list, scorer="WRatio", score_cutoff=0.0, exclude_
     if n_splits is None:
         n_splits = default_splits(n_from, n_grp)
     n_splits = max(1, min(int(n_splits), n_grp))
-    part_idx = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
-    part_score = torch.zeros((n_splits, n_from), dtype=torch.float64, device=dev)
-    part_dist = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
+    shape = (n_splits, n_from) if k is None else (n_splits, n_from, k)
+    part_idx = torch.full(shape, -1, dtype=torch.int32, device=dev)
+    part_score = torch.zeros(shape, dtype=torch.float64, device=dev)
     counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
     fl = np.maximum(np.maximum(F.lens[0], F.lens[1]), F.lens[2])
     classes = np.select([fl <= 64, fl <= 128], [1, 2], 4).astype(np.int32)
@@ -135,8 +129,31 @@ def fuzz_argbest(from_list, to_list, scorer="WRatio", score_cutoff=0.0, exclude_
                 tens += [packs[v][0], packs[v][1], packs[v][2]]
             tens += [d_order, d_tok_blob, d_tok_off, part_idx, part_score, counter, None]
             arr = (ctypes.c_void_p * len(tens))(*[t.data_ptr() if t is not None else 0 for t in tens])
-            _lib.call("pfz_fuzz_argbest", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
-                      int(bool(exclude_self)), int(self_shift), n_splits, _stream())
+            if k is None:
+                _lib.call("pfz_fuzz_argbest", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
+                          int(bool(exclude_self)), int(self_shift), n_splits, _stream())
+            else:
+                _lib.call("pfz_fuzz_topk", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
+                          int(bool(exclude_self)), int(self_shift), n_splits, int(k), _stream())
+    return part_idx, part_score, n_splits, (F, T, packs, keep, d_order, d_tok_blob, d_tok_off)
+
+
+def fuzz_argbest(from_list, to_list, scorer="WRatio", score_cutoff=0.0, exclude_self=False, n_splits=None, self_shift=0,
+                 to_index_base=0):
+    """Best to-string per from-string under a rapidfuzz scorer (scores in [0, 100]).  Returns device tensors
+    (best_idx int32[n_from] (-1: no to-string reached score_cutoff), best_score float64[n_from]).
+    exclude_self skips to-row == from-row + self_shift; to_index_base is added to the returned indices (row-block shards)."""
+    if scorer not in SCORER:
+        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
+    dev = _dev()
+    n_from, n_to = len(from_list), len(to_list)
+    best_idx = torch.full((max(n_from, 1),), -1, dtype=torch.int32, device=dev)
+    best_score = torch.zeros(max(n_from, 1), dtype=torch.float64, device=dev)
+    if n_from == 0 or n_to == 0:
+        return best_idx[:n_from], best_score[:n_from]
+    part_idx, part_score, n_splits, staged = _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift,
+                                                      to_index_base, None)
+    part_dist = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
     best_dist = torch.empty(max(n_from, 1), dtype=torch.int32, device=dev)
     _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx), _p(best_score), _p(best_dist),
               _stream())
@@ -144,3 +161,24 @@ def fuzz_argbest(from_list, to_list, scorer="WRatio", score_cutoff=0.0, exclude_
     if to_index_base:
         best_idx = torch.where(best_idx >= 0, best_idx + int(to_index_base), best_idx)
     return best_idx[:n_from], best_score[:n_from]
+
+
+def fuzz_topk(from_list, to_list, k, scorer="WRatio", score_cutoff=0.0, exclude_self=False, n_splits=None, self_shift=0,
+              to_index_base=0):
+    """The k best to-strings per from-string (1 <= k <= 32) under the candidates and key of fuzz_argbest (score desc, index asc).
+    Returns device tensors (idx int32[n_from, k] (-1: empty slot), score float64[n_from, k] (0.0 in empty slots));
+    exclude_self, self_shift and to_index_base as in fuzz_argbest."""
+    k = check_top_n(k)
+    if scorer not in SCORER:
+        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
+    dev = _dev()
+    n_from, n_to = len(from_list), len(to_list)
+    if n_from == 0 or n_to == 0:
+        return (torch.full((n_from, k), -1, dtype=torch.int32, device=dev), torch.zeros((n_from, k), dtype=torch.float64, device=dev))
+    part_idx, part_score, n_splits, staged = _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift,
+                                                      to_index_base, k)
+    idx, score = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
+    torch.cuda.current_stream().synchronize()                  # the staged host buffers above go out of scope with this call
+    if to_index_base:
+        idx = torch.where(idx >= 0, idx + int(to_index_base), idx)
+    return idx, score

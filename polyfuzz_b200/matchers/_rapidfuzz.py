@@ -14,6 +14,9 @@ published known answers):
                                                                          -> csrc/pfz_lev.cu (K3, Jaro mode)
 A scorer may be given by name or as the rapidfuzz / jellyfish callable of that __name__.  Arbitrary Python callables cannot be
 compiled to the device and raise NotImplementedError -- there is no CPU fallback.
+top_n = k (1..32) returns the k best to-strings per from-string (process.extract(..., limit=k) semantics: score desc, then
+to-index asc) in the columns To, Similarity, To_2, Similarity_2, ...; the reference implements top_n only for TF-IDF and
+Embeddings (polyfuzz/polyfuzz.py:100-102).  top_n = 1 is the arg-best path, unchanged.
 Deviations from the reference, both documented reference bugs (SURVEY.md 8a): a self-match excludes
 index i only (the reference mutates the shared to_list, _rapidfuzz.py:103-104), and the matcher can be
 reused for a two-list call after a self-match (`equal_lists` is per call)."""
@@ -23,8 +26,9 @@ import numpy as np
 import pandas as pd
 
 from ._base import BaseMatcher
+from ._utils import clip_top_n
 from .. import editdist, fuzzy
-from ..distributed import get_comm, shard_bounds
+from ..distributed import get_comm, merge_topk_any, shard_bounds
 
 _NAMES = {"ratio": "ratio", "levenshtein": "norm_lev", "norm_lev": "norm_lev", "normalized_similarity": "norm_lev",
           "normalized_levenshtein": "norm_lev"}
@@ -71,17 +75,51 @@ def _argbest(from_list, targets, metric, cutoff, self_match, distributed):
     return editdist.lev_merge(gi, gs, gd)
 
 
+def _topk(from_list, targets, metric, cutoff, self_match, distributed, k):
+    """Top-k sibling of _argbest: the k best to-strings per from-string (device idx int32[n, k], -1 = empty slot, and score
+    float64[n, k]) on this GPU, or -- distributed=True under torchrun -- per to_list row-block followed by ONE all-gather of the
+    per-shard lists and the canonical merge, as TF-IDF and Embeddings do: all ranks get the single-GPU result."""
+    comm = get_comm() if distributed else None
+    token_scorer = metric in fuzzy.SCORER and metric != "ratio"
+    if comm is None:
+        if token_scorer:
+            return fuzzy.fuzz_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match)
+        return editdist.edit_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match)
+    lo, hi = shard_bounds(len(targets), comm.world_size, comm.rank)
+    if token_scorer:
+        idx, val = fuzzy.fuzz_topk(from_list, targets[lo:hi], k, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
+    else:
+        Q = editdist.EditQueries(from_list)
+        T = editdist.EditTargets(targets[lo:hi])
+        idx, val = editdist.edit_topk_staged(Q, T, k, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
+    gi, gv = comm.all_gather_topk(idx.contiguous(), val.contiguous())
+    return merge_topk_any(gi, gv, k)
+
+
+def _topk_frame(from_list, targets, idx, score):
+    """From, To, Similarity, To_2, Similarity_2, ... from host top-k arrays; scores unrounded, an empty slot is (None, 0.0)."""
+    to_arr = np.empty(len(targets) + 1, dtype=object); to_arr[:-1] = targets; to_arr[-1] = None
+    cols = {"From": pd.Series(list(from_list), dtype=object)}
+    for r in range(idx.shape[1]):
+        filled = idx[:, r] >= 0
+        cols["To" if r == 0 else f"To_{r + 1}"] = pd.Series(to_arr[np.where(filled, idx[:, r], len(targets))], dtype=object)
+        cols["Similarity" if r == 0 else f"Similarity_{r + 1}"] = np.where(filled, score[:, r], 0.0)
+    return pd.DataFrame(cols)
+
+
 def torch_full_like_int(t):
     import torch
     return torch.full_like(t, -1)
 
 class RapidFuzz(BaseMatcher):
     """Edit-distance matcher (GPU).  Arguments as in the reference: n_jobs (accepted, ignored -- the GPU
-    scores all pairs in one launch), score_cutoff in [0,1], scorer (default fuzz.WRatio, as the reference), model_id."""
+    scores all pairs in one launch), score_cutoff in [0,1], scorer (default fuzz.WRatio, as the reference), model_id.
+    top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given."""
 
     def __init__(self, n_jobs: int = 1, score_cutoff: float = 0, scorer: Union[str, Callable] = "WRatio", model_id: str = None,
-                 distributed: bool = False):
+                 distributed: bool = False, top_n: int = 1):
         super().__init__(model_id)
+        self.top_n = editdist.check_top_n(top_n)
         self.type = "EditDistance"
         self.distributed = distributed
         self.score_cutoff = score_cutoff * 100
@@ -92,11 +130,15 @@ class RapidFuzz(BaseMatcher):
 
     def match(self, from_list: List[str], to_list: List[str] = None, **kwargs) -> pd.DataFrame:
         """(from, best to, score/100); no candidate with score >= score_cutoff -> (from, None, 0.0)
-        (polyfuzz/models/_rapidfuzz.py:106-113)."""
+        (polyfuzz/models/_rapidfuzz.py:106-113).  top_n > 1: the k best, an empty slot is (None, 0.0)."""
         self_match = to_list is None
         targets = from_list if self_match else to_list
         scale = 1.0 if self._metric == "norm_lev" else 100.0
         cutoff = self.score_cutoff / 100.0 if self._metric == "norm_lev" else self.score_cutoff
+        top_n = clip_top_n(self.top_n, to_list)
+        if top_n > 1:
+            idx, score = _topk(from_list, targets, self._metric, cutoff, self_match, self.distributed, top_n)
+            return _topk_frame(from_list, targets, idx.cpu().numpy(), score.cpu().numpy() / scale)
         idx, score, _ = _argbest(from_list, targets, self._metric, cutoff, self_match, self.distributed)
         idx = idx.cpu().numpy(); score = score.cpu().numpy() / scale
         to_arr = np.empty(len(targets) + 1, dtype=object); to_arr[:-1] = targets; to_arr[-1] = None
@@ -108,11 +150,16 @@ class RapidFuzz(BaseMatcher):
 class EditDistance(BaseMatcher):
     """Edit-distance matcher with the reference's EditDistance surface (n_jobs, scorer, model_id, normalize):
     Similarity is the scorer's raw value (fuzz.ratio: 0..100, Jaro / Jaro-Winkler: 0..1) of the best to-string,
-    min-max normalised over the column when `normalize` (polyfuzz/models/_distance.py:83-86)."""
+    min-max normalised over the column when `normalize` (polyfuzz/models/_distance.py:83-86).
+    top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given; an empty
+    slot is (None, 0.0).  With top_n > 1, `normalize` takes ONE min and ONE max over every filled Similarity cell of the
+    frame (empty slots excluded), so the first Similarity column can differ from the top_n = 1 frame's, whose min and max
+    cover the best matches only; without `normalize` the first three columns are the top_n = 1 frame."""
 
     def __init__(self, n_jobs: int = 1, scorer: Union[str, Callable] = "ratio", model_id: str = None, normalize: bool = True,
-                 distributed: bool = False):
+                 distributed: bool = False, top_n: int = 1):
         super().__init__(model_id)
+        self.top_n = editdist.check_top_n(top_n)
         self.type = "EditDistance"
         self.distributed = distributed
         self.scorer = scorer
@@ -129,6 +176,16 @@ class EditDistance(BaseMatcher):
         # np.argmax over the scorer's values (polyfuzz/models/_distance.py:98-99): no cutoff; the token scorers take
         # score_cutoff = 0 (their default), which every score passes
         no_cut = 0.0 if self._metric in fuzzy.SCORER and self._metric != "ratio" else float("-inf")
+        top_n = clip_top_n(self.top_n, to_list)
+        if top_n > 1:
+            idx, score = _topk(from_list, targets, self._metric, no_cut, self_match, self.distributed, top_n)
+            idx = idx.cpu().numpy(); score = score.cpu().numpy()
+            if self.normalize:
+                filled = idx >= 0
+                lo, hi = score[filled].min(), score[filled].max()
+                with np.errstate(invalid="ignore", divide="ignore"):
+                    score = np.where(filled, (score - lo) / (hi - lo), 0.0)
+            return _topk_frame(from_list, targets, idx, score)
         idx, score, _ = _argbest(from_list, targets, self._metric, no_cut, self_match, self.distributed)
         idx = idx.cpu().numpy(); score = score.cpu().numpy()
         to_arr = np.empty(len(targets), dtype=object); to_arr[:] = targets
