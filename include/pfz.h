@@ -37,6 +37,8 @@ extern "C" {
 #define PFZ_METRIC_RATIO     3     /* rapidfuzz fuzz.ratio = (1 - indel/(|a|+|b|))*100             */
 #define PFZ_METRIC_JARO      4     /* jellyfish jaro_similarity(from, to), in [0, 1]                */
 #define PFZ_METRIC_JARO_WINKLER 5  /* jellyfish jaro_winkler_similarity(from, to), long_tolerance=False */
+#define PFZ_METRIC_OSA       6     /* optimal string alignment distance (restricted Damerau-Levenshtein) */
+#define PFZ_METRIC_NORM_OSA  7     /* 1 - osa/max(|a|,|b|)                                         */
 
 int         pfz_abi_version(void);
 const char *pfz_last_error(void);
@@ -226,12 +228,15 @@ int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32
 
 /* scores the from-strings listed in from_ids (all of one word class: n_words = 0 -> length <= 32 (one
  * 32-bit word), 1/2/4/8/16 -> length <= 64*n_words) against every to-string.
- *   metric: PFZ_METRIC_*; for NORM_LEV / RATIO / JARO / JARO_WINKLER a candidate needs score >= score_cutoff
+ *   metric: PFZ_METRIC_*; for NORM_LEV / RATIO / JARO / JARO_WINKLER / NORM_OSA a candidate needs score >= score_cutoff
  *   exclude_self: skip to-row == from-row + self_shift
  *   part_*: [n_splits][n_from] partial bests (merge with pfz_lev_merge); ties -> lowest to-index;
  *           part_dist holds the distance, or for JARO / JARO_WINKLER the number of matching characters
- *   matrix (may be NULL): int32 [n_from][matrix_ld] full distance matrix (Levenshtein or Indel); must be
- *           NULL for JARO / JARO_WINKLER
+ *   matrix (may be NULL): int32 [n_from][matrix_ld] full distance matrix (Levenshtein, Indel, or OSA for OSA /
+ *           NORM_OSA); must be NULL for JARO / JARO_WINKLER
+ * OSA / NORM_OSA: optimal string alignment (restricted Damerau-Levenshtein) on code points: insertions, deletions,
+ * substitutions and swaps of two adjacent characters, no substring edited twice (osa("CA", "ABC") = 3, where unrestricted
+ * Damerau-Levenshtein gives 2); DESIGN.md 4.9 gives the recurrence.
  *   counter: int32[n_splits], zeroed by the callee
  * JARO / JARO_WINKLER: jellyfish's definition on code points, from-string first (the reference calls
  * scorer(from_string, to_string), polyfuzz/models/_distance.py:98); DESIGN.md 4.5 gives the recurrence.  */
@@ -248,7 +253,7 @@ int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32
  * to-row == from-row + self_shift excluded when exclude_self) and key (score desc, to-index asc).
  * Replaces: rapidfuzz process.extract(query, to_list, scorer, limit=k), and the sort of the scorer values of
  *           polyfuzz/models/_distance.py:98-99 where the reference takes np.argmax.
- *   metric: NORM_LEV, RATIO, JARO or JARO_WINKLER; there is no distance output and no matrix.
+ *   metric: NORM_LEV, RATIO, JARO, JARO_WINKLER or NORM_OSA; there is no distance output and no matrix.
  *   part_idx / part_score: [n_splits][n_from][k] sorted lists, empty slots (-1, 0.0); merge them with pfz_topk_merge.   */
 int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
                  int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,

@@ -77,10 +77,13 @@ template <> struct WordOps<uint64_t> { static constexpr int BITS = 64; static __
 
 // One warp scores pattern `pat` against every to-string of its split.  LCS = false: Levenshtein (Myers 1999,
 // blocks: Hyyro 2003); LCS = true: longest common subsequence (Hyyro 2004) -> Indel = la + lb - 2*LCS.
+// OSA = true (with LCS = false): optimal string alignment (Hyyro 2003's transposition extension of the same recurrence):
+// D0 and the match masks of the previous text symbol are kept per block, DESIGN.md 4.9.
 // TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings.
 // (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; 0 = unspecified)
-template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false>
+template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false, bool OSA = false>
 __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const LevParams P) {
+    static_assert(!(OSA && LCS), "OSA extends the Levenshtein recurrence");
     constexpr int B = WordOps<W>::BITS;
     extern __shared__ __align__(16) unsigned char dyn[];
     const int lane = lane_id();
@@ -131,8 +134,12 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
             int dist;
             if (!LCS) {
                 W Pv[NW], Mv[NW];
+                W D0[NW], PMo[NW];                                    // OSA: D0 and Peq of the previous text symbol
 #pragma unroll
-                for (int b = 0; b < NW; ++b) { Pv[b] = ~(W)0; Mv[b] = 0; }
+                for (int b = 0; b < NW; ++b) {
+                    Pv[b] = ~(W)0; Mv[b] = 0;
+                    if constexpr (OSA) { D0[b] = 0; PMo[b] = 0; }     // PMo = 0: no transposition at the first symbol
+                }
                 int score = m;
                 uint32_t nextw = nmax > 0 ? src[0] : 0u;
                 for (int j0 = 0; j0 < nmax; j0 += 4) {
@@ -143,23 +150,45 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
                         if (j0 + bb < n) {
                             const int s = (word >> (8 * bb)) & 0xff;
                             int hin = 1;                              // D[0][j] - D[0][j-1] = +1
+                            W trc = 0;                                // OSA: top bit of the block below's X
 #pragma unroll
                             for (int b = 0; b < NW; ++b) {
                                 if (b <= last_blk) {
                                     W Eq = peq[s * NW + b];
                                     const W pv = Pv[b], mv = Mv[b];
-                                    const W Xv = Eq | mv;
-                                    if (hin < 0) Eq |= 1;
-                                    const W Xh = (((Eq & pv) + pv) ^ pv) | Eq;
-                                    W Ph = mv | ~(Xh | pv);
-                                    W Mh = pv & Xh;
-                                    const int top = (b == last_blk) ? last_bit : B - 1;
-                                    const int hout = (int)((Ph >> top) & 1) - (int)((Mh >> top) & 1);
-                                    Ph <<= 1; Mh <<= 1;
-                                    if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
-                                    Pv[b] = Mh | ~(Xv | Ph);
-                                    Mv[b] = Ph & Xv;
-                                    hin = hout;
+                                    if constexpr (!OSA) {
+                                        const W Xv = Eq | mv;
+                                        if (hin < 0) Eq |= 1;
+                                        const W Xh = (((Eq & pv) + pv) ^ pv) | Eq;
+                                        W Ph = mv | ~(Xh | pv);
+                                        W Mh = pv & Xh;
+                                        const int top = (b == last_blk) ? last_bit : B - 1;
+                                        const int hout = (int)((Ph >> top) & 1) - (int)((Mh >> top) & 1);
+                                        Ph <<= 1; Mh <<= 1;
+                                        if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
+                                        Pv[b] = Mh | ~(Xv | Ph);
+                                        Mv[b] = Ph & Xv;
+                                        hin = hout;
+                                    } else {
+                                        // X: rows that match this symbol where the previous column had no diagonal zero;
+                                        // one row up and ANDed with the previous symbol's matches, it marks a swap of b[j-1], b[j]
+                                        const W X = ~D0[b] & Eq;
+                                        const W TR = ((X << 1) | trc) & PMo[b];
+                                        trc = X >> (B - 1);
+                                        PMo[b] = Eq;
+                                        if (hin < 0) Eq |= 1;
+                                        const W D0n = (((Eq & pv) + pv) ^ pv) | Eq | mv | TR;
+                                        W Ph = mv | ~(D0n | pv);
+                                        W Mh = D0n & pv;
+                                        const int top = (b == last_blk) ? last_bit : B - 1;
+                                        const int hout = (int)((Ph >> top) & 1) - (int)((Mh >> top) & 1);
+                                        Ph <<= 1; Mh <<= 1;
+                                        if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
+                                        Pv[b] = Mh | ~(D0n | Ph);
+                                        Mv[b] = Ph & D0n;
+                                        D0[b] = D0n;
+                                        hin = hout;
+                                    }
                                 }
                             }
                             score += hin;                            // horizontal delta of row m
@@ -207,9 +236,12 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
             }
             if (have) {
                 if (P.matrix) P.matrix[(int64_t)i * P.matrix_ld + orig] = dist;
-                const double sc = score_of(P.metric, dist, m, n);
+                // OSA scores like Levenshtein: NORM_OSA takes NORM_LEV's expression and cutoff, raw OSA is a distance
+                const double sc = OSA ? score_of(P.metric == PFZ_METRIC_NORM_OSA ? PFZ_METRIC_NORM_LEV : PFZ_METRIC_LEV, dist, m, n)
+                                      : score_of(P.metric, dist, m, n);
                 bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift);
-                if ((P.metric == PFZ_METRIC_NORM_LEV || P.metric == PFZ_METRIC_RATIO) && !(sc >= P.cutoff)) ok = false;
+                if ((OSA ? P.metric == PFZ_METRIC_NORM_OSA : (P.metric == PFZ_METRIC_NORM_LEV || P.metric == PFZ_METRIC_RATIO)) &&
+                    !(sc >= P.cutoff)) ok = false;
                 if constexpr (TOPK) { cand_s = sc; cand_j = ok ? orig : -1; }
                 else if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = dist; }
             }
@@ -402,11 +434,11 @@ __global__ void lev_merge_kernel(const int32_t *__restrict__ part_idx, const dou
     }
 }
 
-template <typename W, int NW, bool LCS, bool TOPK>
+template <typename W, int NW, bool LCS, bool TOPK, bool OSA = false>
 static int launch_lev(const LevParams &P, int sms, cudaStream_t st) {
     constexpr int WARPS = 4;
     const size_t smem = (size_t)WARPS * 256 * NW * sizeof(W);
-    auto kernel = lev_kernel<W, NW, LCS, WARPS, TOPK>;
+    auto kernel = lev_kernel<W, NW, LCS, WARPS, TOPK, OSA>;
     PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
@@ -441,9 +473,19 @@ static int launch_jaro(const LevParams &P, int sms, cudaStream_t st) {
     return 0;
 }
 
-// word class -> kernel instantiation (the metric picks Levenshtein, Indel or Jaro)
+// word class -> kernel instantiation (the metric picks Levenshtein, Indel, OSA or Jaro)
 template <bool TOPK>
 static int launch_class(const LevParams &P, int n_words, int sms, cudaStream_t st) {
+    if (P.metric == PFZ_METRIC_OSA || P.metric == PFZ_METRIC_NORM_OSA) {
+        switch (n_words) {
+            case 0: return launch_lev<uint32_t, 1, false, TOPK, true>(P, sms, st);
+            case 1: return launch_lev<uint64_t, 1, false, TOPK, true>(P, sms, st);
+            case 2: return launch_lev<uint64_t, 2, false, TOPK, true>(P, sms, st);
+            case 4: return launch_lev<uint64_t, 4, false, TOPK, true>(P, sms, st);
+            case 8: return launch_lev<uint64_t, 8, false, TOPK, true>(P, sms, st);
+            default: return launch_lev<uint64_t, 16, false, TOPK, true>(P, sms, st);
+        }
+    }
     if (P.metric == PFZ_METRIC_JARO || P.metric == PFZ_METRIC_JARO_WINKLER) {
         switch (n_words) {
             case 0: return launch_jaro<uint32_t, 1, TOPK>(P, sms, st);
@@ -489,7 +531,7 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
                     const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
                     int32_t n_splits, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
                     int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_JARO_WINKLER, "pfz_lev_argbest: unknown metric %d", metric);
+    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_OSA, "pfz_lev_argbest: unknown metric %d", metric);
     PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
                 "pfz_lev_argbest: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
     PFZ_REQUIRE(n_splits >= 1, "pfz_lev_argbest: n_splits < 1");
@@ -510,8 +552,8 @@ int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
                  int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
                  const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
                  int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER,
-                "pfz_lev_topk: metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER)", metric);
+    PFZ_REQUIRE((metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER) || metric == PFZ_METRIC_NORM_OSA,
+                "pfz_lev_topk: metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA)", metric);
     PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
                 "pfz_lev_topk: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
     PFZ_REQUIRE(n_splits >= 1, "pfz_lev_topk: n_splits < 1");

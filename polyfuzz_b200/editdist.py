@@ -7,6 +7,9 @@ polyfuzz/models/_distance.py:89-102) and rapidfuzz's published definitions:
     "lev", "indel"  raw distances (best = smallest)
     "jaro"          jellyfish.jaro_similarity(from, to)                          in [0, 1]
     "jaro_winkler"  jellyfish.jaro_winkler_similarity(from, to), long_tolerance=False   in [0, 1]
+    "norm_osa"  OSA.normalized_similarity = 1 - osa/max(|a|,|b|)               in [0, 1]
+    "osa"       raw optimal string alignment distance (restricted Damerau-Levenshtein: adjacent swaps cost 1, no
+                substring is edited twice, so osa("CA", "ABC") = 3 where unrestricted Damerau-Levenshtein gives 2)
 The Jaro metrics are computed on code points, from-string first (the reference calls scorer(from_string, to_string),
 polyfuzz/models/_distance.py:98); their best_dist is the number of matching characters, and they have no distance
 matrix (want_matrix=True raises ValueError).
@@ -24,7 +27,7 @@ from . import _lib
 from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
-METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3, "jaro": 4, "jaro_winkler": 5}
+METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3, "jaro": 4, "jaro_winkler": 5, "osa": 6, "norm_osa": 7}
 JARO_METRICS = ("jaro", "jaro_winkler")
 N_CODE_POINTS = 0x110000
 MAX_LEN = 1024
@@ -181,7 +184,7 @@ def edit_argbest(from_list, to_list, metric="ratio", score_cutoff=0.0, exclude_s
 
 
 TOPK_MAX = 32
-TOPK_METRICS = ("norm_lev", "ratio", "jaro", "jaro_winkler")
+TOPK_METRICS = ("norm_lev", "ratio", "jaro", "jaro_winkler", "norm_osa")
 
 
 def check_top_n(k):

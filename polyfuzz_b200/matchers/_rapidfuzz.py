@@ -12,8 +12,16 @@ published known answers):
   * EditDistance only: "jaro_similarity" / "jaro" and "jaro_winkler_similarity" / "jaro_winkler" (jellyfish's
     definitions with long_tolerance=False, the custom scorer of the reference's tutorial; raw 0..1 scores)
                                                                          -> csrc/pfz_lev.cu (K3, Jaro mode)
-A scorer may be given by name or as the rapidfuzz / jellyfish callable of that __name__.  Arbitrary Python callables cannot be
-compiled to the device and raise NotImplementedError -- there is no CPU fallback.
+  * "osa" / "optimal_string_alignment" / "osa_normalized_similarity" (rapidfuzz.distance.OSA.normalized_similarity: optimal
+    string alignment, i.e. restricted Damerau-Levenshtein -- a swap of two adjacent characters is one edit, no substring is
+    edited twice, so "CA" -> "ABC" costs 3, not unrestricted Damerau-Levenshtein's 2; 0..1 scores like "levenshtein")
+                                                                         -> csrc/pfz_lev.cu (K3, OSA mode)
+A scorer may be given by name or as the rapidfuzz / jellyfish callable of that __name__.  A callable named
+`normalized_similarity` is OSA when a dotted component of its __module__ is "osa" or starts with "osa_" (case-insensitive, e.g.
+rapidfuzz.distance.OSA), and normalised Levenshtein otherwise.  These rules are written from rapidfuzz's documented module layout;
+rapidfuzz is not a dependency, so its callables' actual __name__ / __module__ values are not checked by the tests, which use
+stand-in functions.  Arbitrary Python callables cannot be compiled to the device and raise NotImplementedError -- there is no
+CPU fallback.
 top_n = k (1..32) returns the k best to-strings per from-string (process.extract(..., limit=k) semantics: score desc, then
 to-index asc) in the columns To, Similarity, To_2, Similarity_2, ...; the reference implements top_n only for TF-IDF and
 Embeddings (polyfuzz/polyfuzz.py:100-102).  top_n = 1 is the arg-best path, unchanged.
@@ -31,24 +39,33 @@ from .. import editdist, fuzzy
 from ..distributed import get_comm, merge_topk_any, shard_bounds
 
 _NAMES = {"ratio": "ratio", "levenshtein": "norm_lev", "norm_lev": "norm_lev", "normalized_similarity": "norm_lev",
-          "normalized_levenshtein": "norm_lev"}
+          "normalized_levenshtein": "norm_lev", "osa": "norm_osa", "optimal_string_alignment": "norm_osa",
+          "osa_normalized_similarity": "norm_osa"}
 _FUZZ = {k.lower(): k for k in fuzzy.SCORER if k != "ratio"}
 # jellyfish's function names (and short forms); 0..1 scores, so only EditDistance takes them
 _JARO = {"jaro": "jaro", "jaro_similarity": "jaro", "jaro_winkler": "jaro_winkler", "jaro_winkler_similarity": "jaro_winkler"}
 
 
+def _is_osa_module(module) -> bool:
+    """rapidfuzz.distance.OSA and its implementation modules (OSA_py, OSA_cpp, ...): a dotted component "osa" or "osa_*"."""
+    parts = module.lower().split(".") if isinstance(module, str) else []
+    return any(p == "osa" or p.startswith("osa_") for p in parts)
+
+
 def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
-    """-> "ratio" | "norm_lev" | "jaro" | "jaro_winkler" (K3) or one of fuzzy.SCORER (K3b)."""
+    """-> "ratio" | "norm_lev" | "norm_osa" | "jaro" | "jaro_winkler" (K3) or one of fuzzy.SCORER (K3b)."""
     if scorer is None:
         scorer = default
     key = scorer.lower() if isinstance(scorer, str) else getattr(scorer, "__name__", "").lower()
+    if key == "normalized_similarity" and not isinstance(scorer, str) and _is_osa_module(getattr(scorer, "__module__", None)):
+        return "norm_osa"
     if key in _NAMES:
         return _NAMES[key]
     if key in _FUZZ:
         return _FUZZ[key]
     if allow_jaro and key in _JARO:
         return _JARO[key]
-    raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: 'ratio', 'levenshtein', "
+    raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: 'ratio', 'levenshtein', 'osa', "
                               f"{sorted(_FUZZ.values())}" + (", 'jaro_similarity', 'jaro_winkler_similarity'" if allow_jaro else "")
                               + "); polyfuzz_b200 has no CPU fallback")
 
@@ -133,8 +150,9 @@ class RapidFuzz(BaseMatcher):
         (polyfuzz/models/_rapidfuzz.py:106-113).  top_n > 1: the k best, an empty slot is (None, 0.0)."""
         self_match = to_list is None
         targets = from_list if self_match else to_list
-        scale = 1.0 if self._metric == "norm_lev" else 100.0
-        cutoff = self.score_cutoff / 100.0 if self._metric == "norm_lev" else self.score_cutoff
+        unit = self._metric in ("norm_lev", "norm_osa")                        # scores already on 0..1
+        scale = 1.0 if unit else 100.0
+        cutoff = self.score_cutoff / 100.0 if unit else self.score_cutoff
         top_n = clip_top_n(self.top_n, to_list)
         if top_n > 1:
             idx, score = _topk(from_list, targets, self._metric, cutoff, self_match, self.distributed, top_n)
@@ -149,7 +167,7 @@ class RapidFuzz(BaseMatcher):
 
 class EditDistance(BaseMatcher):
     """Edit-distance matcher with the reference's EditDistance surface (n_jobs, scorer, model_id, normalize):
-    Similarity is the scorer's raw value (fuzz.ratio: 0..100, Jaro / Jaro-Winkler: 0..1) of the best to-string,
+    Similarity is the scorer's raw value (fuzz.ratio: 0..100, Levenshtein / OSA / Jaro / Jaro-Winkler: 0..1) of the best to-string,
     min-max normalised over the column when `normalize` (polyfuzz/models/_distance.py:83-86).
     top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given; an empty
     slot is (None, 0.0).  With top_n > 1, `normalize` takes ONE min and ONE max over every filled Similarity cell of the
