@@ -182,8 +182,11 @@ int pfz_spcos_topk(const int32_t *a_indptr, const int32_t *a_indices, const doub
  *            4 m + 2 units for a from-row of m terms; tile must be a multiple of 256) or 32 (one per word, unit 2^-26, margin 1e-5).
  *   nnz_cap_from: capacity of a_indices / a_data (>= nnz).  ws: >= pfz_spcos_block_ws_bytes(...) bytes (clustering keys, block
  *            tables, and 192 candidate slots per (split, from-row)).
- *   Output as pfz_spcos_topk: [n_splits][n_from][k] partial lists (pfz_topk_merge when n_splits > 1).                    */
+ *   Output as pfz_spcos_topk: [n_splits][n_from][k] partial lists (pfz_topk_merge when n_splits > 1).
+ * pfz_spcos_block_gcnt_offset: byte offset in ws of int32 gcnt[n_splits][n_from], the candidates each (split, from-row) left
+ *   for exact re-scoring in the last call (a diagnostic: how much the filter let through).                                 */
 int64_t pfz_spcos_block_ws_bytes(int32_t n_from, int64_t nnz_cap_from, int32_t n_vocab, int32_t n_splits);
+int64_t pfz_spcos_block_gcnt_offset(int32_t n_from, int64_t nnz_cap_from, int32_t n_vocab, int32_t n_splits);
 int pfz_index_pack_q26(const uint16_t *post_idx, const double *post_val, const int32_t *nnz_dev, void *post_pk, void *stream);
 int pfz_index_pack_q15(const uint16_t *post_idx, const double *post_val, const int32_t *nnz_dev, int32_t tile, void *post_pk, void *stream);
 int pfz_spcos_topk_block(const int32_t *a_indptr, const int32_t *a_indices, const double *a_data, int32_t n_from, int64_t nnz_cap_from,

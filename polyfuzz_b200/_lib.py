@@ -33,6 +33,7 @@ _PROTOS = {
     "pfz_spcos_topk_hash": [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i64, c_i32,
                             c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_spcos_block_ws_bytes": [c_i32, c_i64, c_i32, c_i32],
+    "pfz_spcos_block_gcnt_offset": [c_i32, c_i64, c_i32, c_i32],
     "pfz_index_pack_q26": [c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_index_pack_q15": [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp],
     "pfz_spcos_topk_block": [c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32,
@@ -62,6 +63,7 @@ _PROTOS = {
     "pfz_dense_topn_select": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp],
 }
 _RESTYPES = {"pfz_last_error": ctypes.c_char_p, "pfz_scan_ws_bytes": c_i64, "pfz_launch_count": c_i64, "pfz_spcos_block_ws_bytes": c_i64,
+             "pfz_spcos_block_gcnt_offset": c_i64,
              "pfz_dense_exact_fallback_ws_bytes": c_i64}
 
 

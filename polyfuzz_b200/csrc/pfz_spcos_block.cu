@@ -779,13 +779,18 @@ struct ExactParams {
     int64_t from_base, to_base; int32_t *top_idx; double *top_val;
 };
 constexpr int EX_ROW_CAP = 128;                  // from-row terms staged in shared memory (the block kernel's contract; longer rows take the generic merge)
+constexpr int EX_HASH = 2 * EX_ROW_CAP;          // open-addressed table of the staged from-row: load factor <= 1/2
+__device__ __forceinline__ unsigned ex_slot(int t) { return ((unsigned)t * 0x9E3779B1u) >> 24; }   // (EX_HASH = 256 slots)
+constexpr int EX_CHUNK = 8;                      // to-row entries loaded per step (independent loads)
 __global__ void __launch_bounds__(256) blk_exact_kernel(const ExactParams P) {
-    // The from-row is staged once per warp in shared memory; every lane scores one candidate: it walks ITS to-row (entries loaded
-    // four at a time, independent loads) and finds each term in the from-row by binary search -- the same number of steps in every
-    // lane, so the warp does not diverge as it does in a two-pointer merge.  Common terms are met in ascending order and the
-    // products are rounded before the add: the canonical fp64 score, bit for bit.
-    __shared__ int s_ai[8][EX_ROW_CAP];
-    __shared__ double s_av[8][EX_ROW_CAP];
+    // The from-row is staged once per warp in a shared-memory hash table (term -> weight, linear probing); every lane scores one
+    // candidate: it walks ITS to-row (entries loaded EX_CHUNK at a time, independent loads) and looks each term up in the table --
+    // about 1.5 probes on average, where a binary search over the row took ceil(log2(m + 1)) dependent shared-memory loads.
+    // Common terms are met in ascending order (the to-row's) and the products are rounded before the add: the canonical fp64
+    // score, bit for bit.
+    static_assert(EX_HASH == 256, "ex_slot() yields 8 bits");
+    __shared__ int s_hk[8][EX_HASH];
+    __shared__ double s_hv[8][EX_HASH];
     const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
     const int64_t gw = (int64_t)blockIdx.x * 8 + wl;
     if (gw >= (int64_t)P.n_splits * P.n_from) return;
@@ -802,11 +807,17 @@ __global__ void __launch_bounds__(256) blk_exact_kernel(const ExactParams P) {
     if (m > EX_ROW_CAP) {
         blk_exact_rounds(P.a_indptr, P.a_indices, P.a_data, P.b_indptr, P.b_indices, P.b_data, P.to_base, K, row, self_loc, cand, n, tv, ti, kv, ki);
     } else {
-        int *ai = s_ai[wl]; double *av = s_av[wl];
-        for (int e = lane; e < m; e += 32) { ai[e] = P.a_indices[a0 + e]; av[e] = P.a_data[a0 + e]; }
+        int *hk = s_hk[wl]; double *hv = s_hv[wl];
+        for (int s2 = lane; s2 < EX_HASH; s2 += 32) hk[s2] = -1;
         __syncwarp();
-        int steps = 0;
-        while ((1 << steps) <= m) ++steps;                           // binary-search steps for m entries: ceil(log2(m + 1))
+        for (int e = lane; e < m; e += 32) {                          // the row's terms are distinct: a slot is taken once
+            const int t = P.a_indices[a0 + e];
+            const double x = P.a_data[a0 + e];
+            unsigned sl = ex_slot(t);
+            while (atomicCAS(&hk[sl], -1, t) != -1) sl = (sl + 1) & (EX_HASH - 1);
+            hv[sl] = x;
+        }
+        __syncwarp();
         kv = shfl_d(tv, K - 1); ki = __shfl_sync(FULL, ti, K - 1);
         int left = n;
         while (left > 0) {
@@ -815,15 +826,17 @@ __global__ void __launch_bounds__(256) blk_exact_kernel(const ExactParams P) {
             if (lane < n_round) {
                 const int jloc = cand[off + lane];
                 const int b0 = P.b_indptr[jloc], b1 = P.b_indptr[jloc + 1];
-                for (int q = b0; q < b1; q += 4) {
-                    int t[4]; double wgt[4];
+                for (int q = b0; q < b1; q += EX_CHUNK) {
+                    int t[EX_CHUNK]; double wgt[EX_CHUNK];
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) { t[u] = 0x7fffffff; wgt[u] = 0.0; if (q + u < b1) { t[u] = P.b_indices[q + u]; wgt[u] = P.b_data[q + u]; } }
+                    for (int u = 0; u < EX_CHUNK; ++u) { t[u] = -1; wgt[u] = 0.0; if (q + u < b1) { t[u] = P.b_indices[q + u]; wgt[u] = P.b_data[q + u]; } }
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        int lo = 0, hi = m;
-                        for (int st = 0; st < steps; ++st) { const int mid = (lo + hi) >> 1; if (lo < hi) { if (ai[mid] < t[u]) lo = mid + 1; else hi = mid; } }
-                        if (lo < m && ai[lo] == t[u]) sc = __dadd_rn(sc, __dmul_rn(av[lo], wgt[u]));
+                    for (int u = 0; u < EX_CHUNK; ++u) {
+                        if (t[u] < 0) break;                                // (past the end of the to-row)
+                        unsigned sl = ex_slot(t[u]);
+                        int k;
+                        while ((k = hk[sl]) != t[u] && k != -1) sl = (sl + 1) & (EX_HASH - 1);
+                        if (k == t[u]) sc = __dadd_rn(sc, __dmul_rn(hv[sl], wgt[u]));
                     }
                 }
                 j = (int)(P.to_base + jloc);
@@ -910,6 +923,10 @@ extern "C" {
 
 int64_t pfz_spcos_block_ws_bytes(int32_t n_from, int64_t nnz_cap_from, int32_t n_vocab, int32_t n_splits) {
     return (int64_t)block_ws_layout(n_from, nnz_cap_from, n_vocab, n_splits).total;
+}
+
+int64_t pfz_spcos_block_gcnt_offset(int32_t n_from, int64_t nnz_cap_from, int32_t n_vocab, int32_t n_splits) {
+    return (int64_t)block_ws_layout(n_from, nnz_cap_from, n_vocab, n_splits).gcnt;
 }
 
 int pfz_index_pack_q26(const uint16_t *post_idx, const double *post_val, const int32_t *nnz_dev, void *post_pk, void *stream) {

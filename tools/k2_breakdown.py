@@ -6,9 +6,12 @@ Runs the bench.py step (K1 + index + K2, the L2 flushed before every step, `--wa
   * the card: name, power limit, current and maximum SM clock;
   * the step time from CUDA events (profiler off);
   * per-kernel device times from torch.profiler, in a run of its own (summed over the profiled steps, divided by --steps);
+  * the candidates the block kernel's filter left per from-row for exact re-scoring (its `gcnt` array): mean and maximum,
+    to set against tools/k2_cand_count.py (the numbers differ somewhat: fixed point and group order);
   * with --timing-lib (a library built with PFZ_NVCC_EXTRA=-DPFZ_B3_TIMING), the block kernel's per-phase split of SM
     cycles, measured in a subprocess that loads that library.
---lib loads another build of libpfz.so instead of the package's (A/B of two builds in one session).
+--lib loads another build of libpfz.so instead of the package's (A/B of two builds in one session); entry points that build
+does not have are left out.
 """
 import argparse
 import ctypes
@@ -45,6 +48,9 @@ def setup(args):
     from polyfuzz_b200 import _lib
     if args.lib:
         _lib._LIB_PATH = os.path.abspath(args.lib)
+        other = ctypes.CDLL(_lib._LIB_PATH)
+        for name in [n for n in _lib._PROTOS if not hasattr(other, n)]:
+            del _lib._PROTOS[name]
     import torch
     from polyfuzz_b200 import datasets, engine
     from polyfuzz_b200.distributed import tfidf_topk_sharded
@@ -61,6 +67,40 @@ def setup(args):
         out["r"] = tfidf_topk_sharded(vec, staged, staged, 0, 10, 0.0, self_match=True, from_index_base=0, fit=True,
                                       fit_on_from=False, comm=None, n_docs_total=len(names))
     return torch, step, flush, kind, out
+
+
+def candidate_counts(torch, step, flush):
+    """gcnt of one step: the block kernel's workspace is kept while the call runs and read back afterwards."""
+    from polyfuzz_b200 import _lib, engine
+    lib = _lib.load()
+    orig_block, orig_ws = engine._spcos_block, engine._ws
+    seen = []
+
+    def block(a, index, k, *rest):
+        kept = []
+        engine._ws = lambda nbytes: kept.append(orig_ws(nbytes)) or kept[-1]
+        try:
+            r = orig_block(a, index, k, *rest)
+        finally:
+            engine._ws = orig_ws
+        n_from, n_splits = a.n_rows, rest[-1]
+        shape = (n_from, int(a.indices.numel()), index.n_vocab, n_splits)
+        if hasattr(lib, "pfz_spcos_block_gcnt_offset"):
+            off = lib.pfz_spcos_block_gcnt_offset(*shape)
+        else:                          # older builds: gcnt, then 192 candidate slots per entry, end the workspace
+            a256 = lambda x: (x + 255) // 256 * 256  # noqa: E731
+            off = lib.pfz_spcos_block_ws_bytes(*shape) - a256(n_splits * n_from * 192 * 4) - a256(n_splits * n_from * 4)
+        seen.append((kept[0], off, n_splits * n_from))
+        return r
+
+    engine._spcos_block = block
+    try:
+        flush.zero_(); step()
+        torch.cuda.synchronize()
+    finally:
+        engine._spcos_block = orig_block
+    g = torch.cat([ws[off:off + 4 * n].view(torch.int32).to(torch.int64) for ws, off, n in seen])
+    return {"rows": int(g.numel()), "mean": round(float(g.double().mean()), 3), "max": int(g.max())}
 
 
 def run_phases(args):
@@ -102,6 +142,8 @@ def main():
         ms.append(e0.elapsed_time(e1))
     rec["step_ms"] = [round(v, 3) for v in ms]
     rec["tile"] = out["r"][3].tile
+    rec["gcnt"] = candidate_counts(torch, step, flush)
+    print(f"candidates left for exact re-scoring per from-row (gcnt): mean {rec['gcnt']['mean']}, max {rec['gcnt']['max']}")
     # per-kernel device times: a run of its own, the profiler on
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
