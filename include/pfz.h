@@ -39,6 +39,8 @@ extern "C" {
 #define PFZ_METRIC_JARO_WINKLER 5  /* jellyfish jaro_winkler_similarity(from, to), long_tolerance=False */
 #define PFZ_METRIC_OSA       6     /* optimal string alignment distance (restricted Damerau-Levenshtein) */
 #define PFZ_METRIC_NORM_OSA  7     /* 1 - osa/max(|a|,|b|)                                         */
+#define PFZ_METRIC_DL        8     /* unrestricted Damerau-Levenshtein distance (pfz_dl_* only)    */
+#define PFZ_METRIC_NORM_DL   9     /* 1 - dl/max(|a|,|b|)                   (pfz_dl_* only)        */
 
 int         pfz_abi_version(void);
 const char *pfz_last_error(void);
@@ -263,6 +265,28 @@ int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
                  const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
                  int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
                  int32_t k, int32_t *part_idx, double *part_score, int32_t *counter, void *stream);
+
+/* Unrestricted Damerau-Levenshtein (Lowrance-Wagner with unit costs, on code points): the fewest insertions, deletions,
+ * substitutions and swaps of two adjacent characters, where a swapped pair may be edited again (dl("CA", "ABC") = 2).
+ * Same parameters, layout, candidates, key and outputs as pfz_lev_argbest / pfz_lev_topk, plus
+ *   gate (may be NULL): float64[n_from], per from-row a proven lower bound of its k-th best score (k = 1 for the arg-best) over
+ *         the whole to-list; pairs whose score upper bound is below it are skipped.  The k-th best OSA score of the row (the
+ *         pfz_lev_* pass with OSA / NORM_OSA and the same cutoff, exclusion and k, merged over the splits) is such a bound, and a
+ *         row with fewer than k OSA candidates takes score_cutoff (NORM_DL) or -inf (DL).  NULL: no gate.
+ *   metric: DL (raw distance, best = smallest, no cutoff; arg-best only) or NORM_DL (1 - dl/max(|a|,|b|), score >= score_cutoff).
+ *   matrix (arg-best only, may be NULL): DL distances of every pair; requires gate == NULL.
+ * DESIGN.md 4.10 gives the bounds and the kernel. */
+int pfz_dl_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                   int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
+                   const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
+                   int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
+                   int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
+                   const double *gate, int32_t *counter, void *stream);
+int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
+                const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
+                int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
+                int32_t k, int32_t *part_idx, double *part_score, const double *gate, int32_t *counter, void *stream);
 
 /* K3b  rapidfuzz's token / partial / weighted scorers with a fused per-row arg-best (csrc/pfz_fuzz.cu).
  * Replaces: process.extractOne(query, to_list, scorer=fuzz.WRatio | partial_ratio | token_*_ratio | ..., score_cutoff) at

@@ -15,6 +15,7 @@
 // Patterns of <= 32 symbols use 32-bit words (half the integer work), <= 64 one 64-bit word, longer ones
 // NW 64-bit blocks with horizontal carries (Hyyro 2003).  Work is integer-ALU bound (SURVEY.md 8d).
 #include "pfz_common.cuh"
+#include <math_constants.h>
 
 namespace pfz {
 
@@ -510,6 +511,288 @@ static int launch_class(const LevParams &P, int n_words, int sms, cudaStream_t s
 #undef PFZ_LEV_CASE
 }
 
+// ---- unrestricted Damerau-Levenshtein (DESIGN.md 4.10) ------------------------------------------------------------------
+// Per pair the warp computes OSA bit-parallel (the recurrence of lev_kernel<..., OSA = true>), which brackets DL:
+//     max(ceil(2*osa/3), |m - n|) <= dl <= osa.
+// A pair whose score upper bound is below the row's gate (a proven lower bound of its k-th best score) or below the running
+// k-th exact score is dropped; if the two bounds meet the score is exact; otherwise the pair is queued, and every 32 queued
+// pairs (and at the end of the row) all lanes run the exact DP, one pair each.  Matrix mode runs the DP on every pair.
+constexpr int DL_NONE = 32000;          // RK: no earlier text occurrence (larger than any real term: distances are <= j + m)
+
+template <typename W, int NW>
+struct DlLayout {                       // one warp's shared memory
+    static constexpr int MAXM = WordOps<W>::BITS * NW;
+    static constexpr size_t PEQ = (size_t)256 * NW * sizeof(W);
+    static constexpr size_t QUEUE = 32 * sizeof(int2);                                  // (sorted to-position, lower bound)
+    static constexpr size_t STATE = (size_t)3 * (MAXM + 1) * 32 * sizeof(int16_t);      // A, P2, RK: [row][lane]
+    static constexpr size_t PAT = (MAXM + 1 + 15) / 16 * 16;                            // pattern symbols, 1-based
+    static constexpr size_t PER_WARP = PEQ + QUEUE + STATE + PAT;
+};
+
+// Exact unrestricted Damerau-Levenshtein (Lowrance-Wagner, unit costs) of pat[1..m] against the lane's text (n symbols in the
+// packed column src), streamed column by column over the text with O(m) state.  A transposition block whose gaps on both
+// sides are >= 1 costs 1 + ga + gb >= 2 + max(ga, gb), which substitutions and indels already reach, so only two block shapes
+// are needed (Zhao & Sahni 2019):
+//   text gap 0    (a[i] = b[j-1]):  d[l-1][j-2] + (i - l),  l = last pattern row < i with a[l] = b[j]   -> L (register)
+//   pattern gap 0 (a[i-1] = b[j]):  d[i-2][k-1] + (j - k),  k = last text column < j with b[k] = a[i]  -> RK[i] = d[i-2][k-1] - k
+// A holds d[.][j-1] below row i and d[.][j] above it, P2 likewise d[.][j-2] / d[.][j-1]; both are stored relative to their
+// column (d[r][c] - c lies in [-m, m]), so int16 fits every pattern length.  Rows are 32 lanes apart (conflict-free).
+// Symbol 0 (text-only code points) equals nothing.
+__device__ __forceinline__ int dl_dp(const uint8_t *__restrict__ pat, int m, const uint32_t *__restrict__ src, int n,
+                                  int16_t *A, int16_t *P2, int16_t *RK) {
+    if (m == 0) return n;
+    for (int r = 0; r <= m; ++r) { A[r * 32] = (int16_t)r; P2[r * 32] = 0; RK[r * 32] = DL_NONE; }
+    int bprev = 0, last = m;
+    uint32_t word = 0;
+    for (int j = 1; j <= n; ++j) {
+        if (((j - 1) & 3) == 0) word = src[(size_t)((j - 1) >> 2) * 32];
+        const int bj = (word >> (8 * ((j - 1) & 3))) & 0xff;
+        int up = j, diag = j - 1, pdiag = 0, ap = 0;
+        int L = 1 << 28;                                       // no row l < i with a[l] = b[j] yet
+        for (int i = 1; i <= m; ++i) {
+            const int ai = pat[i];
+            const int left = A[i * 32] + (j - 1);
+            const int p2 = P2[(i - 1) * 32] + (j - 2);
+            const bool eq = bj != 0 && ai == bj;
+            int d = min(diag + (eq ? 0 : 1), min(up, left) + 1);
+            if (bprev != 0 && ai == bprev) d = min(d, L + i);
+            if (ap != 0 && ap == bj) d = min(d, RK[i * 32] + j);
+            if (eq) {
+                L = p2 - i;
+                if (i >= 2) RK[i * 32] = (int16_t)(pdiag - j);
+            }
+            P2[(i - 1) * 32] = (int16_t)(diag - (j - 1));
+            A[i * 32] = (int16_t)(d - j);
+            pdiag = diag; diag = left; up = d; ap = ai;
+        }
+        P2[m * 32] = (int16_t)(diag - (j - 1));
+        bprev = bj;
+        last = up;
+    }
+    return last;
+}
+
+template <typename W, int NW, int WARPS, bool TOPK>
+__global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, const double *__restrict__ gate) {
+    constexpr int B = WordOps<W>::BITS;
+    using Lay = DlLayout<W, NW>;
+    extern __shared__ __align__(16) unsigned char dyn[];
+    const int lane = lane_id();
+    const int w = threadIdx.x >> 5;
+    unsigned char *base = dyn + (size_t)w * Lay::PER_WARP;
+    W *peq = reinterpret_cast<W *>(base);                                    // peq[sym * NW + block]
+    int2 *queue = reinterpret_cast<int2 *>(base + Lay::PEQ);
+    int16_t *sA = reinterpret_cast<int16_t *>(base + Lay::PEQ + Lay::QUEUE) + lane;
+    int16_t *sP2 = sA + (Lay::MAXM + 1) * 32, *sRK = sP2 + (Lay::MAXM + 1) * 32;
+    uint8_t *pat = base + Lay::PEQ + Lay::QUEUE + Lay::STATE;
+    const bool norm = P.metric == PFZ_METRIC_NORM_DL;
+    const bool full = P.matrix != nullptr;                                  // matrix mode: the DP on every pair
+    const double NEG_INF = -CUDART_INF;
+    const int split = blockIdx.y;
+    const int n_grp = (P.n_to + 31) >> 5;
+    const int per = (n_grp + P.n_splits - 1) / P.n_splits;
+    const int g_lo = split * per, g_hi = min(n_grp, g_lo + per);
+    int32_t *counter = P.counter + split;
+
+    for (;;) {
+        int q = 0;
+        if (lane == 0) q = atomicAdd(counter, 1);
+        q = __shfl_sync(FULL, q, 0);
+        if (q >= P.n_ids) break;
+        const int i = P.from_ids[q];
+        const int64_t fb = P.from_off[i];
+        const int m = (int)(P.from_off[i + 1] - fb);
+        for (int e = lane; e < 256 * NW; e += 32) peq[e] = 0;
+        __syncwarp();
+        for (int p = lane; p < m; p += 32) {
+            const uint32_t c = P.from_blob[fb + p];
+            const int s = c < 0x110000u ? P.sym_table[c] : 0;
+            pat[p + 1] = (uint8_t)s;
+            if (s) {
+                if (sizeof(W) == 8) atomicOr(reinterpret_cast<unsigned long long *>(&peq[s * NW + p / B]), 1ull << (p % B));
+                else atomicOr(reinterpret_cast<unsigned *>(&peq[s * NW + p / B]), 1u << (p % B));
+            }
+        }
+        __syncwarp();
+        const int last_bit = (m - 1) & (B - 1);
+        const int last_blk = m > 0 ? (m - 1) / B : 0;
+        const double gt = gate ? gate[i] : NEG_INF;
+
+        double best_s = 0.0; int best_j = -1, best_d = -1;
+        WarpTopK top;
+        if constexpr (TOPK) top.init(P.k);
+        double kth = NEG_INF;                                               // warp-uniform running k-th exact score
+        int qn = 0;                                                         // warp-uniform queue fill
+
+        auto score = [&](int d, int n) { return norm ? score_of(PFZ_METRIC_NORM_LEV, d, m, n) : -(double)d; };
+        auto offer = [&](bool have, int d, int n, int orig) {
+            double sc = 0.0; int cj = -1;
+            if (have) {
+                sc = score(d, n);
+                const bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) && !(norm && !(sc >= P.cutoff));
+                if (ok) cj = orig;
+            }
+            if constexpr (TOPK) {
+                top.offer(sc, cj);
+                const double ts = shfl_d(top.s, P.k - 1);
+                kth = __shfl_sync(FULL, top.j, P.k - 1) >= 0 ? ts : NEG_INF;
+            } else {
+                if (cj >= 0 && (best_j < 0 || sc > best_s || (sc == best_s && cj < best_j))) { best_s = sc; best_j = cj; best_d = d; }
+                double v = best_j >= 0 ? best_s : NEG_INF;
+#pragma unroll
+                for (int o = 16; o; o >>= 1) v = fmax(v, shfl_d(v, lane ^ o));
+                kth = v;
+            }
+        };
+        // all lanes: lane r < cnt takes queue entry r, re-tests it against the threshold (which may have risen since it was
+        // queued) and runs the DP
+        auto flush = [&](int cnt) {
+            const bool act = lane < cnt;
+            const int2 e = act ? queue[lane] : make_int2(0, 0);
+            const int n = act ? P.slen[e.x] : 0;
+            const int orig = act ? P.sorig[e.x] : -1;
+            const bool run = act && (full || !(score(e.y, n) < fmax(gt, kth)));
+            int d = 0;
+            if (run) d = dl_dp(pat, m, P.packed + P.grp_word_off[e.x >> 5] + (e.x & 31), n, sA, sP2, sRK);
+            if (run && full) P.matrix[(int64_t)i * P.matrix_ld + orig] = d;
+            offer(run, d, n, orig);
+        };
+
+        for (int g = g_lo; g < g_hi; ++g) {
+            const int p = g * 32 + lane;
+            const bool have = p < P.n_to;
+            const int n = have ? P.slen[p] : 0;
+            const int orig = have ? P.sorig[p] : -1;
+            int nmax = n;
+#pragma unroll
+            for (int d = 16; d; d >>= 1) nmax = max(nmax, __shfl_xor_sync(FULL, nmax, d));
+            const uint32_t *src = P.packed + P.grp_word_off[g] + lane;
+            // OSA, bit-parallel: lev_kernel's OSA recurrence (DESIGN.md 4.9)
+            W Pv[NW], Mv[NW], D0[NW], PMo[NW];
+#pragma unroll
+            for (int b = 0; b < NW; ++b) { Pv[b] = ~(W)0; Mv[b] = 0; D0[b] = 0; PMo[b] = 0; }
+            int score_m = m;
+            uint32_t nextw = nmax > 0 ? src[0] : 0u;
+            for (int j0 = 0; j0 < nmax; j0 += 4) {
+                const uint32_t word = nextw;
+                if (j0 + 4 < nmax) nextw = src[(size_t)((j0 >> 2) + 1) * 32];
+#pragma unroll
+                for (int bb = 0; bb < 4; ++bb) {
+                    if (j0 + bb < n) {
+                        const int s = (word >> (8 * bb)) & 0xff;
+                        int hin = 1;
+                        W trc = 0;
+#pragma unroll
+                        for (int b = 0; b < NW; ++b) {
+                            if (b <= last_blk) {
+                                W Eq = peq[s * NW + b];
+                                const W pv = Pv[b], mv = Mv[b];
+                                const W X = ~D0[b] & Eq;
+                                const W TR = ((X << 1) | trc) & PMo[b];
+                                trc = X >> (B - 1);
+                                PMo[b] = Eq;
+                                if (hin < 0) Eq |= 1;
+                                const W D0n = (((Eq & pv) + pv) ^ pv) | Eq | mv | TR;
+                                W Ph = mv | ~(D0n | pv);
+                                W Mh = D0n & pv;
+                                const int top_bit = (b == last_blk) ? last_bit : B - 1;
+                                const int hout = (int)((Ph >> top_bit) & 1) - (int)((Mh >> top_bit) & 1);
+                                Ph <<= 1; Mh <<= 1;
+                                if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
+                                Pv[b] = Mh | ~(D0n | Ph);
+                                Mv[b] = Ph & D0n;
+                                D0[b] = D0n;
+                                hin = hout;
+                            }
+                        }
+                        score_m += hin;
+                    }
+                }
+            }
+            const int osa = m > 0 ? score_m : n;
+            const int lb = max((2 * osa + 2) / 3, abs(m - n));
+            const bool excl = P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift;
+            bool direct = false, queued = false;
+            if (have && full) queued = true;
+            else if (have && !excl) {
+                const double ub = score(lb, n);
+                if (!(ub < fmax(gt, kth)) && !(norm && ub < P.cutoff)) {
+                    if (lb == osa) direct = true; else queued = true;
+                }
+            }
+            if (__any_sync(FULL, direct)) offer(direct, osa, n, orig);
+            const unsigned need = __ballot_sync(FULL, queued);
+            if (need) {
+                const int pos = qn + __popc(need & ((1u << lane) - 1u));
+                if (queued && pos < 32) queue[pos] = make_int2(p, lb);
+                int tot = qn + __popc(need);
+                if (tot >= 32) {
+                    __syncwarp();
+                    flush(32);
+                    __syncwarp();
+                    if (queued && pos >= 32) queue[pos - 32] = make_int2(p, lb);
+                    tot -= 32;
+                }
+                qn = tot;
+                __syncwarp();
+            }
+        }
+        if (qn > 0) flush(qn);
+
+        if constexpr (TOPK) {
+            const size_t o = ((size_t)split * P.n_from + i) * P.k;
+            top.store(P.part_idx + o, P.part_score + o);
+        } else {
+#pragma unroll
+            for (int d = 16; d; d >>= 1) {
+                const double os = shfl_d(best_s, lane ^ d);
+                const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
+                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
+            }
+            if (lane == 0) {
+                const size_t o = (size_t)split * P.n_from + i;
+                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// Shared memory per warp (DlLayout): 7.6 KB at 32 symbols, 15 KB at 64, ..., 225 KB at 1 024 -- 4 warps per CTA up to 128
+// symbols, 2 at 256, 1 from 512 on.
+template <typename W, int NW, bool TOPK>
+static int launch_dl(const LevParams &P, const double *gate, int sms, cudaStream_t st) {
+    using Lay = DlLayout<W, NW>;
+    constexpr size_t SMEM_MAX = 227 * 1024;
+    static_assert(Lay::PER_WARP % 16 == 0 && Lay::PER_WARP <= SMEM_MAX, "DL state does not fit one warp's shared memory");
+    constexpr int WARPS = Lay::PER_WARP * 4 <= SMEM_MAX ? 4 : Lay::PER_WARP * 2 <= SMEM_MAX ? 2 : 1;
+    const size_t smem = (size_t)WARPS * Lay::PER_WARP;
+    auto kernel = dl_kernel<W, NW, WARPS, TOPK>;
+    PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int occ = 0;
+    PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
+    if (occ < 1) occ = 1;
+    int gx = sms * occ;
+    const int need = (P.n_ids + WARPS - 1) / WARPS;
+    if (gx > need) gx = need;
+    if (gx < 1) gx = 1;
+    kernel<<<dim3(gx, P.n_splits), WARPS * 32, smem, st>>>(P, gate);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
+template <bool TOPK>
+static int launch_dl_class(const LevParams &P, const double *gate, int n_words, int sms, cudaStream_t st) {
+    switch (n_words) {
+        case 0: return launch_dl<uint32_t, 1, TOPK>(P, gate, sms, st);
+        case 1: return launch_dl<uint64_t, 1, TOPK>(P, gate, sms, st);
+        case 2: return launch_dl<uint64_t, 2, TOPK>(P, gate, sms, st);
+        case 4: return launch_dl<uint64_t, 4, TOPK>(P, gate, sms, st);
+        case 8: return launch_dl<uint64_t, 8, TOPK>(P, gate, sms, st);
+        default: return launch_dl<uint64_t, 16, TOPK>(P, gate, sms, st);
+    }
+}
+
 }  // namespace pfz
 
 using namespace pfz;
@@ -567,6 +850,47 @@ int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
     LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
                 exclude_self, self_shift, n_splits, part_idx, part_score, nullptr, nullptr, 0, n_from, counter, k};
     return launch_class<true>(P, n_words, sms, st);
+}
+
+int pfz_dl_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                   int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                   const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                   int32_t n_splits, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
+                   const double *gate, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(metric == PFZ_METRIC_DL || metric == PFZ_METRIC_NORM_DL, "pfz_dl_argbest: metric %d unsupported (DL, NORM_DL)", metric);
+    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_dl_argbest: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
+    PFZ_REQUIRE(n_splits >= 1, "pfz_dl_argbest: n_splits < 1");
+    PFZ_REQUIRE(!(matrix && gate), "pfz_dl_argbest: the distance matrix needs every pair, so gate must be NULL with a matrix");
+    if (n_ids <= 0 || n_to < 0) return 0;
+    cudaStream_t st = as_stream(stream);
+    int dev = 0, sms = 0;
+    PFZ_CUDA_OK(cudaGetDevice(&dev));
+    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
+    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
+                exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter, 1};
+    return launch_dl_class<false>(P, gate, n_words, sms, st);
+}
+
+int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, const double *gate, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(metric == PFZ_METRIC_NORM_DL, "pfz_dl_topk: metric %d unsupported (NORM_DL)", metric);
+    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_dl_topk: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
+    PFZ_REQUIRE(n_splits >= 1, "pfz_dl_topk: n_splits < 1");
+    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_dl_topk: k=%d unsupported (1..32)", k);
+    if (n_ids <= 0 || n_to < 0) return 0;
+    cudaStream_t st = as_stream(stream);
+    int dev = 0, sms = 0;
+    PFZ_CUDA_OK(cudaGetDevice(&dev));
+    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
+    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
+                exclude_self, self_shift, n_splits, part_idx, part_score, nullptr, nullptr, 0, n_from, counter, k};
+    return launch_dl_class<true>(P, gate, n_words, sms, st);
 }
 
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits, int32_t n_from,

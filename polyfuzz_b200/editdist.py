@@ -10,6 +10,9 @@ polyfuzz/models/_distance.py:89-102) and rapidfuzz's published definitions:
     "norm_osa"  OSA.normalized_similarity = 1 - osa/max(|a|,|b|)               in [0, 1]
     "osa"       raw optimal string alignment distance (restricted Damerau-Levenshtein: adjacent swaps cost 1, no
                 substring is edited twice, so osa("CA", "ABC") = 3 where unrestricted Damerau-Levenshtein gives 2)
+    "norm_dl"   DamerauLevenshtein.normalized_similarity = 1 - dl/max(|a|,|b|)  in [0, 1]
+    "dl"        raw unrestricted Damerau-Levenshtein distance (Lowrance-Wagner, unit costs: a swapped pair may be edited
+                again, so dl("CA", "ABC") = 2); computed by pfz_dl_*, gated by an OSA pass (DESIGN.md 4.10)
 The Jaro metrics are computed on code points, from-string first (the reference calls scorer(from_string, to_string),
 polyfuzz/models/_distance.py:98); their best_dist is the number of matching characters, and they have no distance
 matrix (want_matrix=True raises ValueError).
@@ -27,8 +30,11 @@ from . import _lib
 from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
-METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3, "jaro": 4, "jaro_winkler": 5, "osa": 6, "norm_osa": 7}
+METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3, "jaro": 4, "jaro_winkler": 5, "osa": 6, "norm_osa": 7, "dl": 8,
+          "norm_dl": 9}
 JARO_METRICS = ("jaro", "jaro_winkler")
+# DL metric -> the OSA metric whose k-th best score gates it (norm_osa <= norm_dl pair by pair, DESIGN.md 4.10)
+DL_GATE = {"dl": "osa", "norm_dl": "norm_osa"}
 N_CODE_POINTS = 0x110000
 MAX_LEN = 1024
 
@@ -137,10 +143,17 @@ def default_splits(n_from, n_grp):
     return max(1, min(n_grp, (want + max(n_from, 1) - 1) // max(n_from, 1)))
 
 
+def _gate_fill(metric, score_cutoff):
+    """Gate of a row with fewer than k OSA candidates: the cutoff (norm_dl), or no bound (raw dl has no cutoff)."""
+    return float(score_cutoff) if metric == "norm_dl" else float("-inf")
+
+
 def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, want_matrix=False,
-                        n_splits=None, to_index_base=0):
+                        n_splits=None, to_index_base=0, dl_gate=True):
     """Kernels only.  Returns (best_idx int32[n_from] (-1 = none; + to_index_base otherwise), best_score float64[n_from],
-    best_dist int32[n_from] [, matrix int32[n_from, n_to]]) as device tensors."""
+    best_dist int32[n_from] [, matrix int32[n_from, n_to]]) as device tensors.
+    dl / norm_dl: per word class an OSA arg-best pass and its split merge give each row's gate, then pfz_dl_argbest;
+    dl_gate=False (for timing) skips the OSA pass, and a matrix is computed without it."""
     if want_matrix and metric in JARO_METRICS:
         raise ValueError(f"want_matrix=True: the {metric!r} metric has no integer distance matrix")
     dev = _dev()
@@ -159,9 +172,25 @@ def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=Fal
     part_score = torch.zeros((n_splits, n_from), dtype=torch.float64, device=dev)
     part_dist = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
     counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
+    dl = metric in DL_GATE
     for d_table, groups in Q.batches:
         _lib.call("pfz_lev_pack", _p(T.d_blob), _p(T.d_off), _p(T.d_order), n_to, _p(d_table), _p(T.d_goff), _p(T.packed), _p(T.slen), _stream())
         for nw, d_ids, n_ids in groups:
+            if dl:
+                gate = None
+                if dl_gate and not want_matrix:
+                    _lib.call("pfz_lev_argbest", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
+                              _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[DL_GATE[metric]], float(score_cutoff),
+                              int(bool(exclude_self)), int(self_shift), n_splits, _p(part_idx), _p(part_score), _p(part_dist), None, 0,
+                              _p(counter), _stream())
+                    _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx),
+                              _p(best_score), _p(best_dist), _stream())
+                    gate = torch.where(best_idx >= 0, best_score, _gate_fill(metric, score_cutoff))
+                _lib.call("pfz_dl_argbest", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
+                          _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)),
+                          int(self_shift), n_splits, _p(part_idx), _p(part_score), _p(part_dist), _p(matrix),
+                          int(matrix.stride(0)) if matrix is not None else 0, _p(gate), _p(counter), _stream())
+                continue
             _lib.call("pfz_lev_argbest", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
                       _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)),
                       int(self_shift), n_splits, _p(part_idx), _p(part_score), _p(part_dist), _p(matrix),
@@ -175,16 +204,16 @@ def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=Fal
 
 
 def edit_argbest(from_list, to_list, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0,
-                 want_matrix=False, n_splits=None):
+                 want_matrix=False, n_splits=None, dl_gate=True):
     """Host lists in, device tensors out (see edit_argbest_staged)."""
     _dev()
     Q = EditQueries(from_list)
     T = EditTargets(to_list)
-    return edit_argbest_staged(Q, T, metric, score_cutoff, exclude_self, self_shift, want_matrix, n_splits)
+    return edit_argbest_staged(Q, T, metric, score_cutoff, exclude_self, self_shift, want_matrix, n_splits, dl_gate=dl_gate)
 
 
 TOPK_MAX = 32
-TOPK_METRICS = ("norm_lev", "ratio", "jaro", "jaro_winkler", "norm_osa")
+TOPK_METRICS = ("norm_lev", "ratio", "jaro", "jaro_winkler", "norm_osa", "norm_dl")
 
 
 def check_top_n(k):
@@ -194,10 +223,13 @@ def check_top_n(k):
     return int(k)
 
 
-def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, to_index_base=0):
+def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, to_index_base=0,
+                     dl_gate=True):
     """Kernels only: the k best to-strings per from-string (pfz_lev_topk, then pfz_topk_merge over the to-splits), with the
     candidates and the key of edit_argbest_staged.  Returns device (idx int32[n_from, k] (-1 = empty slot; + to_index_base
-    otherwise), score float64[n_from, k] (0.0 in empty slots))."""
+    otherwise), score float64[n_from, k] (0.0 in empty slots)).
+    norm_dl: per word class a norm_osa top-k pass and its split merge give each row's gate (its k-th best OSA score), then
+    pfz_dl_topk; dl_gate=False (for timing) skips the OSA pass."""
     k = check_top_n(k)
     if metric not in TOPK_METRICS:
         raise ValueError(f"top-k is available for the metrics {TOPK_METRICS}, not {metric!r}")
@@ -214,6 +246,18 @@ def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=Fal
     for d_table, groups in Q.batches:
         _lib.call("pfz_lev_pack", _p(T.d_blob), _p(T.d_off), _p(T.d_order), n_to, _p(d_table), _p(T.d_goff), _p(T.packed), _p(T.slen), _stream())
         for nw, d_ids, n_ids in groups:
+            if metric in DL_GATE:
+                gate = None
+                if dl_gate:
+                    _lib.call("pfz_lev_topk", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
+                              _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[DL_GATE[metric]], float(score_cutoff),
+                              int(bool(exclude_self)), int(self_shift), n_splits, k, _p(part_idx), _p(part_score), _p(counter), _stream())
+                    gi, gs = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
+                    gate = torch.where(gi[:, k - 1] >= 0, gs[:, k - 1], _gate_fill(metric, score_cutoff)).contiguous()
+                _lib.call("pfz_dl_topk", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
+                          _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)), int(self_shift),
+                          n_splits, k, _p(part_idx), _p(part_score), _p(gate), _p(counter), _stream())
+                continue
             _lib.call("pfz_lev_topk", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
                       _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)), int(self_shift),
                       n_splits, k, _p(part_idx), _p(part_score), _p(counter), _stream())
@@ -223,13 +267,13 @@ def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=Fal
     return idx, score
 
 
-def edit_topk(from_list, to_list, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None):
+def edit_topk(from_list, to_list, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, dl_gate=True):
     """Host lists in, device tensors out (see edit_topk_staged)."""
     k = check_top_n(k)
     _dev()
     Q = EditQueries(from_list)
     T = EditTargets(to_list)
-    return edit_topk_staged(Q, T, k, metric, score_cutoff, exclude_self, self_shift, n_splits)
+    return edit_topk_staged(Q, T, k, metric, score_cutoff, exclude_self, self_shift, n_splits, dl_gate=dl_gate)
 
 
 def lev_merge(part_idx, part_score, part_dist):

@@ -16,9 +16,16 @@ published known answers):
     string alignment, i.e. restricted Damerau-Levenshtein -- a swap of two adjacent characters is one edit, no substring is
     edited twice, so "CA" -> "ABC" costs 3, not unrestricted Damerau-Levenshtein's 2; 0..1 scores like "levenshtein")
                                                                          -> csrc/pfz_lev.cu (K3, OSA mode)
+  * "dl" / "unrestricted_damerau_levenshtein" / "damerau_levenshtein_normalized_similarity" (unrestricted Damerau-Levenshtein,
+    rapidfuzz.distance.DamerauLevenshtein's metric: a swapped pair may be edited again, so "CA" -> "ABC" costs 2;
+    1 - dl / max(|a|, |b|), 0..1 scores like "levenshtein")             -> csrc/pfz_lev.cu (K3, dl_kernel, gated by OSA)
+The bare name "damerau_levenshtein" raises NotImplementedError: some libraries mean OSA by it, others unrestricted DL, so the
+user picks "osa" or "dl".
 A scorer may be given by name or as the rapidfuzz / jellyfish callable of that __name__.  A callable named
 `normalized_similarity` is OSA when a dotted component of its __module__ is "osa" or starts with "osa_" (case-insensitive, e.g.
-rapidfuzz.distance.OSA), and normalised Levenshtein otherwise.  These rules are written from rapidfuzz's documented module layout;
+rapidfuzz.distance.OSA), and normalised Levenshtein otherwise -- including rapidfuzz.distance.DamerauLevenshtein's, which
+therefore scores Levenshtein, not DL; pointing it at "dl" changes what an existing call returns, so it is left to a separate
+fix.  These rules are written from rapidfuzz's documented module layout;
 rapidfuzz is not a dependency, so its callables' actual __name__ / __module__ values are not checked by the tests, which use
 stand-in functions.  Arbitrary Python callables cannot be compiled to the device and raise NotImplementedError -- there is no
 CPU fallback.
@@ -40,7 +47,8 @@ from ..distributed import get_comm, merge_topk_any, shard_bounds
 
 _NAMES = {"ratio": "ratio", "levenshtein": "norm_lev", "norm_lev": "norm_lev", "normalized_similarity": "norm_lev",
           "normalized_levenshtein": "norm_lev", "osa": "norm_osa", "optimal_string_alignment": "norm_osa",
-          "osa_normalized_similarity": "norm_osa"}
+          "osa_normalized_similarity": "norm_osa", "dl": "norm_dl", "unrestricted_damerau_levenshtein": "norm_dl",
+          "damerau_levenshtein_normalized_similarity": "norm_dl"}
 _FUZZ = {k.lower(): k for k in fuzzy.SCORER if k != "ratio"}
 # jellyfish's function names (and short forms); 0..1 scores, so only EditDistance takes them
 _JARO = {"jaro": "jaro", "jaro_similarity": "jaro", "jaro_winkler": "jaro_winkler", "jaro_winkler_similarity": "jaro_winkler"}
@@ -53,7 +61,7 @@ def _is_osa_module(module) -> bool:
 
 
 def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
-    """-> "ratio" | "norm_lev" | "norm_osa" | "jaro" | "jaro_winkler" (K3) or one of fuzzy.SCORER (K3b)."""
+    """-> "ratio" | "norm_lev" | "norm_osa" | "norm_dl" | "jaro" | "jaro_winkler" (K3) or one of fuzzy.SCORER (K3b)."""
     if scorer is None:
         scorer = default
     key = scorer.lower() if isinstance(scorer, str) else getattr(scorer, "__name__", "").lower()
@@ -65,7 +73,10 @@ def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
         return _FUZZ[key]
     if allow_jaro and key in _JARO:
         return _JARO[key]
-    raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: 'ratio', 'levenshtein', 'osa', "
+    if key == "damerau_levenshtein":
+        raise NotImplementedError(f"scorer {scorer!r} is ambiguous: use 'osa' (optimal string alignment, restricted "
+                                  "Damerau-Levenshtein) or 'dl' (unrestricted Damerau-Levenshtein)")
+    raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: 'ratio', 'levenshtein', 'osa', 'dl', "
                               f"{sorted(_FUZZ.values())}" + (", 'jaro_similarity', 'jaro_winkler_similarity'" if allow_jaro else "")
                               + "); polyfuzz_b200 has no CPU fallback")
 
@@ -150,7 +161,7 @@ class RapidFuzz(BaseMatcher):
         (polyfuzz/models/_rapidfuzz.py:106-113).  top_n > 1: the k best, an empty slot is (None, 0.0)."""
         self_match = to_list is None
         targets = from_list if self_match else to_list
-        unit = self._metric in ("norm_lev", "norm_osa")                        # scores already on 0..1
+        unit = self._metric in ("norm_lev", "norm_osa", "norm_dl")             # scores already on 0..1
         scale = 1.0 if unit else 100.0
         cutoff = self.score_cutoff / 100.0 if unit else self.score_cutoff
         top_n = clip_top_n(self.top_n, to_list)
@@ -167,7 +178,7 @@ class RapidFuzz(BaseMatcher):
 
 class EditDistance(BaseMatcher):
     """Edit-distance matcher with the reference's EditDistance surface (n_jobs, scorer, model_id, normalize):
-    Similarity is the scorer's raw value (fuzz.ratio: 0..100, Levenshtein / OSA / Jaro / Jaro-Winkler: 0..1) of the best to-string,
+    Similarity is the scorer's raw value (fuzz.ratio: 0..100, Levenshtein / OSA / DL / Jaro / Jaro-Winkler: 0..1) of the best to-string,
     min-max normalised over the column when `normalize` (polyfuzz/models/_distance.py:83-86).
     top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given; an empty
     slot is (None, 0.0).  With top_n > 1, `normalize` takes ONE min and ONE max over every filled Similarity cell of the
