@@ -1,4 +1,5 @@
-// pfz_common.cuh -- shared helpers for libpfz.so (sm_90a only).
+// pfz_common.cuh -- shared helpers for libpfz.so (sm_90a only), among them the row driver of K3 and K3b: split_groups,
+// claim_row, build_peq, the WarpTopK / WarpArgBest epilogues, start_rows and launch_rows.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -87,6 +88,96 @@ struct WarpTopK {
         if (lane < k) { idx[lane] = j; val[lane] = j >= 0 ? s : 0.0; }
     }
 };
+
+// One warp's arg-best under WarpTopK's key: each lane keeps the best (s, j) it was offered (cj < 0: none) and, with DIST, the
+// distance that came with it; store() reduces the warp in a butterfly (the first maximal score = the lowest index among the
+// maxima) and lane 0 writes the row's slot (-1, 0.0, -1 when empty).
+template <bool DIST = true>
+struct WarpArgBest {
+    double s; int j; int d;
+    __device__ __forceinline__ void init() { s = 0.0; j = -1; d = -1; }
+    __device__ __forceinline__ void offer(double cs, int cj, int cd = -1) {
+        if (cj >= 0 && (j < 0 || WarpTopK::before(cs, cj, s, j))) { s = cs; j = cj; if constexpr (DIST) d = cd; }
+    }
+    __device__ __forceinline__ void store(int32_t *idx, double *val, int32_t *dist) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            const double os = shfl_d(s, lane_id() ^ o);
+            const int oj = __shfl_xor_sync(FULL, j, o);
+            offer(os, oj, DIST ? __shfl_xor_sync(FULL, d, o) : -1);
+        }
+        if (lane_id() == 0) {
+            *idx = j; *val = j >= 0 ? s : 0.0;
+            if constexpr (DIST) *dist = d;
+        }
+    }
+};
+
+// ---- K3 / K3b row driver: one warp per from-row, the to-list in groups of 32 split over blockIdx.y ----------------------------
+// the to-groups [lo, hi) of this block's split
+struct GroupRange { int lo, hi; };
+__device__ __forceinline__ GroupRange split_groups(int n_to, int n_splits) {
+    const int n_grp = (n_to + 31) >> 5;
+    const int per = (n_grp + n_splits - 1) / n_splits;
+    const int lo = blockIdx.y * per;
+    return {lo, min(n_grp, lo + per)};
+}
+
+// the warp's next from-row (from_ids[q], q from the split's counter), or -1 once all n_ids rows are taken
+__device__ __forceinline__ int claim_row(int32_t *counter, const int32_t *from_ids, int n_ids) {
+    int q = 0;
+    if (lane_id() == 0) q = atomicAdd(counter, 1);
+    q = __shfl_sync(FULL, q, 0);
+    return q < n_ids ? from_ids[q] : -1;
+}
+
+// One warp's match masks: peq[sym * NW + block] bit p is set where pattern symbol p is sym.  cps: the m code points, mapped by
+// sym_table (symbol 0, the text-only code points, matches nothing); pat (optional) receives the symbols 1-based.
+template <typename W, int NW>
+__device__ __forceinline__ void build_peq(W *peq, const uint32_t *cps, int m, const uint8_t *sym_table, uint8_t *pat = nullptr) {
+    constexpr int B = 8 * sizeof(W);
+    for (int e = lane_id(); e < 256 * NW; e += 32) peq[e] = 0;
+    __syncwarp();
+    for (int p = lane_id(); p < m; p += 32) {
+        const uint32_t c = cps[p];
+        const int s = c < 0x110000u ? sym_table[c] : 0;
+        if (pat) pat[p + 1] = (uint8_t)s;
+        if (s) {
+            if (sizeof(W) == 8) atomicOr(reinterpret_cast<unsigned long long *>(&peq[s * NW + p / B]), 1ull << (p % B));
+            else atomicOr(reinterpret_cast<unsigned *>(&peq[s * NW + p / B]), 1u << (p % B));
+        }
+    }
+    __syncwarp();
+}
+
+// warps per CTA (4, 2 or 1) for a kernel whose warps each take per_warp bytes of shared memory, within budget bytes per CTA
+constexpr int warps_within(size_t per_warp, size_t budget) { return per_warp * 4 <= budget ? 4 : per_warp * 2 <= budget ? 2 : 1; }
+
+// SM count of the current device, and the per-split row counters zeroed on st
+static inline int start_rows(int32_t *counter, int n_splits, cudaStream_t st, int *sms) {
+    int dev = 0;
+    PFZ_CUDA_OK(cudaGetDevice(&dev));
+    PFZ_CUDA_OK(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
+    return 0;
+}
+
+// Launch a row-driver kernel on (gx, n_splits) CTAs of `warps` warps: as many CTAs per split as fit the SMs at once, and no
+// more than n_ids rows need.
+template <typename Kernel, typename... Args>
+static int launch_rows(Kernel kernel, int warps, size_t smem, int n_ids, int n_splits, int sms, cudaStream_t st, const Args &...args) {
+    PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int occ = 0;
+    PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, warps * 32, smem));
+    if (occ < 1) occ = 1;
+    int gx = sms * occ;
+    const int need = (n_ids + warps - 1) / warps;
+    if (gx > need) gx = need;
+    if (gx < 1) gx = 1;
+    kernel<<<dim3(gx, n_splits), warps * 32, smem, st>>>(args...);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
 
 // exclusive scan of int32 -> int32 on a stream; ws from pfz_scan_ws_bytes(n)
 int scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t n, void *ws, cudaStream_t st);

@@ -8,7 +8,7 @@
 // The scorer definitions (incl. the order of the double-precision operations and the way score_cutoff is threaded through
 // WRatio) are those of rapidfuzz 3.x as restated and pinned on rapidfuzz's published known answers in oracle/fuzz.py.
 //
-// Mapping (as K3, pfz_lev.cu): one warp = one from-string, whose bit-vector match masks Peq[symbol] live in shared memory
+// Mapping (as K3, pfz_lev.cu, and with its row driver from pfz_common.cuh): one warp = one from-string, whose bit-vector match masks Peq[symbol] live in shared memory
 // for THREE derived patterns -- a itself, S(a) = its whitespace tokens sorted and joined, U(a) = its distinct tokens sorted and
 // joined; one lane = one to-string at a time (to-strings pre-sorted by length, groups of 32, transposed, 4 byte-symbols per
 // word), with the same three variants b, S(b), U(b).  Every Indel distance is a bit-parallel LCS (Hyyro 2004):
@@ -220,36 +220,20 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
     const int lane = lane_id();
     const int w = threadIdx.x >> 5;
     uint64_t *peq_all = reinterpret_cast<uint64_t *>(dyn) + (size_t)w * 3 * 256 * NW;      // peq[variant][sym * NW + block]
-    const int split = blockIdx.y;
-    const int n_grp = (P.n_to + 31) >> 5;
-    const int per = (n_grp + P.n_splits - 1) / P.n_splits;
-    const int g_lo = split * per, g_hi = min(n_grp, g_lo + per);
-    int32_t *counter = P.counter + split;
     const int sc_id = P.scorer;
     const bool need_sorted = sc_id == FZ_TSORT || sc_id == FZ_TRATIO || sc_id == FZ_PTSORT || sc_id == FZ_PTRATIO || sc_id == FZ_WRATIO;
     const bool need_uniq = sc_id == FZ_TSET || sc_id == FZ_TRATIO || sc_id == FZ_PTSET || sc_id == FZ_PTRATIO || sc_id == FZ_WRATIO;
 
     for (;;) {
-        int q = 0;
-        if (lane == 0) q = atomicAdd(counter, 1);
-        q = __shfl_sync(FULL, q, 0);
-        if (q >= P.n_ids) break;
-        const int i = P.from_ids[q];
+        const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
+        if (i < 0) break;
+        const GroupRange gr = split_groups(P.n_to, P.n_splits);    // per row: held across rows, it adds spills (2 words)
         int lens[3];
         for (int v = 0; v < 3; ++v) {
             const int64_t fb = P.F.off[v][i];
-            const int m = (int)(P.F.off[v][i + 1] - fb);
-            lens[v] = m;
-            uint64_t *peq = peq_all + (size_t)v * 256 * NW;
+            lens[v] = (int)(P.F.off[v][i + 1] - fb);
             if ((v == 1 && !need_sorted) || (v == 2 && !need_uniq)) continue;
-            for (int e = lane; e < 256 * NW; e += 32) peq[e] = 0;
-            __syncwarp();
-            for (int p = lane; p < m; p += 32) {
-                const uint32_t c = P.F.blob[v][fb + p];
-                const int s = c < 0x110000u ? P.sym_table[c] : 0;
-                if (s) atomicOr(reinterpret_cast<unsigned long long *>(&peq[s * NW + p / 64]), 1ull << (p % 64));
-            }
-            __syncwarp();
+            build_peq<uint64_t, NW>(peq_all + (size_t)v * 256 * NW, P.F.blob[v] + fb, lens[v], P.sym_table);
         }
         const int la = lens[0], las = lens[1], lau = lens[2];
         const int32_t *atok = P.F.tok_ids + P.F.tok_ptr[i];
@@ -258,10 +242,10 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
         const uint64_t asig = P.F.sig[i];
         const uint64_t *peq0 = peq_all, *peq1 = peq_all + 256 * NW, *peq2 = peq_all + 2 * 256 * NW;
 
-        double best_s = 0.0; int best_j = -1;
+        WarpArgBest<false> best;
         WarpTopK top;
-        if constexpr (TOPK) top.init(P.k);
-        for (int g = g_lo; g < g_hi; ++g) {
+        if constexpr (TOPK) top.init(P.k); else best.init();
+        for (int g = gr.lo; g < gr.hi; ++g) {
             double cand_s = 0.0; int cand_j = -1;
             do {
                 const int p = g * 32 + lane;
@@ -351,25 +335,16 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
                     }
                 }
                 if constexpr (TOPK) { if (sc >= P.cutoff) { cand_s = sc; cand_j = orig; } }
-                else if (sc >= P.cutoff && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; }
+                else if (sc >= P.cutoff) best.offer(sc, orig);
             } while (0);
             if constexpr (TOPK) top.offer(cand_s, cand_j);
         }
         if constexpr (TOPK) {
-            const size_t o = ((size_t)split * P.n_from + i) * P.k;
+            const size_t o = ((size_t)blockIdx.y * P.n_from + i) * P.k;
             top.store(P.part_idx + o, P.part_score + o);
         } else {
-            // first maximal score = lowest original index among the maxima
-#pragma unroll
-            for (int d = 16; d; d >>= 1) {
-                const double os = shfl_d(best_s, lane ^ d);
-                const int oj = __shfl_xor_sync(FULL, best_j, d);
-                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; }
-            }
-            if (lane == 0) {
-                const size_t o = (size_t)split * P.n_from + i;
-                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0;
-            }
+            const size_t o = (size_t)blockIdx.y * P.n_from + i;
+            best.store(P.part_idx + o, P.part_score + o, nullptr);
         }
         __syncwarp();
     }
@@ -378,19 +353,7 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
 template <int NW, bool TOPK>
 static int launch_fuzz(const FuzzParams &P, int sms, cudaStream_t st) {
     constexpr int WARPS = NW == 1 ? 4 : NW == 2 ? 2 : 1;
-    const size_t smem = (size_t)WARPS * 3 * 256 * NW * 8;
-    auto kernel = fuzz_kernel<NW, WARPS, TOPK>;
-    PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 0;
-    PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
-    if (occ < 1) occ = 1;
-    int gx = sms * occ;
-    const int need = (P.n_ids + WARPS - 1) / WARPS;
-    if (gx > need) gx = need;
-    if (gx < 1) gx = 1;
-    kernel<<<dim3(gx, P.n_splits), WARPS * 32, smem, st>>>(P);
-    PFZ_LAUNCH_OK();
-    return 0;
+    return launch_rows(fuzz_kernel<NW, WARPS, TOPK>, WARPS, (size_t)WARPS * 3 * 256 * NW * 8, P.n_ids, P.n_splits, sms, st, P);
 }
 
 // the 38 pointers of the C ABI (order: include/pfz.h) -> FuzzParams; part_idx / part_score as the caller's entry point lays them out
@@ -398,9 +361,6 @@ template <bool TOPK>
 static int run_fuzz(const void *const *ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
                     double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k_out, void *stream) {
     cudaStream_t st = as_stream(stream);
-    int dev = 0, sms = 0;
-    PFZ_CUDA_OK(cudaGetDevice(&dev));
-    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     FuzzParams P;
     int k = 0;
     auto side = [&](FuzzSide &S) {
@@ -416,7 +376,8 @@ static int run_fuzz(const void *const *ptrs, int32_t n_from, int32_t n_ids, int3
     k++;                                                                            // 38: reserved
     P.n_ids = n_ids; P.n_to = n_to; P.scorer = scorer; P.cutoff = score_cutoff; P.exclude_self = exclude_self; P.self_shift = self_shift;
     P.n_splits = n_splits; P.n_from = n_from; P.k = k_out;
-    PFZ_CUDA_OK(cudaMemsetAsync(P.counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
+    int sms = 0;
+    if (start_rows(P.counter, n_splits, st, &sms)) return 1;
     if (n_words == 1) return launch_fuzz<1, TOPK>(P, sms, st);
     if (n_words == 2) return launch_fuzz<2, TOPK>(P, sms, st);
     return launch_fuzz<4, TOPK>(P, sms, st);

@@ -14,6 +14,10 @@
 //
 // Patterns of <= 32 symbols use 32-bit words (half the integer work), <= 64 one 64-bit word, longer ones
 // NW 64-bit blocks with horizontal carries (Hyyro 2003).  Work is integer-ALU bound (SURVEY.md 8d).
+//
+// Shared by the kernels here: the row driver of pfz_common.cuh (split_groups, claim_row, build_peq, WarpArgBest / WarpTopK,
+// launch_rows), LevColumn (the Levenshtein / OSA column step of lev_kernel and dl_kernel), for_each_text_symbol (the text
+// loop), dispatch_words (n_words -> <W, NW>) and run_k3 (the body of the C entry points).
 #include "pfz_common.cuh"
 #include <math_constants.h>
 
@@ -72,14 +76,105 @@ __device__ __forceinline__ double score_of(int metric, int d, int la, int lb) {
     return -(double)d;                  // raw distances: best = smallest
 }
 
+// the row's slot of part_*: its k best (TOPK) or its arg-best
+template <bool TOPK>
+__device__ __forceinline__ void store_row(const LevParams &P, int i, const WarpTopK &top, WarpArgBest<> &best) {
+    if constexpr (TOPK) {
+        const size_t o = ((size_t)blockIdx.y * P.n_from + i) * P.k;
+        top.store(P.part_idx + o, P.part_score + o);
+    } else {
+        const size_t o = (size_t)blockIdx.y * P.n_from + i;
+        best.store(P.part_idx + o, P.part_score + o, P.part_dist + o);
+    }
+}
+
 template <typename W> struct WordOps;
 template <> struct WordOps<uint32_t> { static constexpr int BITS = 32; static __device__ __forceinline__ int pop(uint32_t x) { return __popc(x); } };
 template <> struct WordOps<uint64_t> { static constexpr int BITS = 64; static __device__ __forceinline__ int pop(uint64_t x) { return __popcll(x); } };
 
-// One warp scores pattern `pat` against every to-string of its split.  LCS = false: Levenshtein (Myers 1999,
-// blocks: Hyyro 2003); LCS = true: longest common subsequence (Hyyro 2004) -> Indel = la + lb - 2*LCS.
-// OSA = true (with LCS = false): optimal string alignment (Hyyro 2003's transposition extension of the same recurrence):
-// D0 and the match masks of the previous text symbol are kept per block, DESIGN.md 4.9.
+// Calls f(symbol) for the n symbols of the lane's to-string (packed column src, 4 symbols per word).  The trip count is the
+// warp's longest string, so the loop is warp-uniform, and the next word is loaded one word ahead: the recurrences f runs are
+// long dependent chains.
+template <typename F>
+__device__ __forceinline__ void for_each_text_symbol(const uint32_t *src, int n, F &&f) {
+    int nmax = n;
+#pragma unroll
+    for (int d = 16; d; d >>= 1) nmax = max(nmax, __shfl_xor_sync(FULL, nmax, d));
+    uint32_t nextw = nmax > 0 ? src[0] : 0u;
+    for (int j0 = 0; j0 < nmax; j0 += 4) {
+        const uint32_t word = nextw;
+        if (j0 + 4 < nmax) nextw = src[(size_t)((j0 >> 2) + 1) * 32];
+#pragma unroll
+        for (int bb = 0; bb < 4; ++bb) {
+            if (j0 + bb < n) f((int)((word >> (8 * bb)) & 0xff));
+        }
+    }
+}
+
+// One bit-parallel column of Levenshtein (Myers 1999, blocks: Hyyro 2003) or, with OSA, of optimal string alignment (Hyyro
+// 2003's transposition extension: D0 and the match masks of the previous text symbol are kept per block, DESIGN.md 4.9).
+// step() takes the text symbol's match masks peq[s * NW ..] and returns the horizontal delta of pattern row m.
+template <typename W, int NW, bool OSA>
+struct LevColumn {
+    static constexpr int B = WordOps<W>::BITS;
+    W Pv[NW], Mv[NW];
+    W D0[NW], PMo[NW];                                    // OSA: D0 and Peq of the previous text symbol
+    __device__ __forceinline__ void init() {
+#pragma unroll
+        for (int b = 0; b < NW; ++b) {
+            Pv[b] = ~(W)0; Mv[b] = 0;
+            if constexpr (OSA) { D0[b] = 0; PMo[b] = 0; }     // PMo = 0: no transposition at the first symbol
+        }
+    }
+    __device__ __forceinline__ int step(const W *eq, int last_blk, int last_bit) {
+        int hin = 1;                                      // D[0][j] - D[0][j-1] = +1
+        W trc = 0;                                        // OSA: top bit of the block below's X
+#pragma unroll
+        for (int b = 0; b < NW; ++b) {
+            if (b <= last_blk) {
+                W Eq = eq[b];
+                const W pv = Pv[b], mv = Mv[b];
+                if constexpr (!OSA) {
+                    const W Xv = Eq | mv;
+                    if (hin < 0) Eq |= 1;
+                    const W Xh = (((Eq & pv) + pv) ^ pv) | Eq;
+                    W Ph = mv | ~(Xh | pv);
+                    W Mh = pv & Xh;
+                    const int top = (b == last_blk) ? last_bit : B - 1;
+                    const int hout = (int)((Ph >> top) & 1) - (int)((Mh >> top) & 1);
+                    Ph <<= 1; Mh <<= 1;
+                    if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
+                    Pv[b] = Mh | ~(Xv | Ph);
+                    Mv[b] = Ph & Xv;
+                    hin = hout;
+                } else {
+                    // X: rows that match this symbol where the previous column had no diagonal zero;
+                    // one row up and ANDed with the previous symbol's matches, it marks a swap of b[j-1], b[j]
+                    const W X = ~D0[b] & Eq;
+                    const W TR = ((X << 1) | trc) & PMo[b];
+                    trc = X >> (B - 1);
+                    PMo[b] = Eq;
+                    if (hin < 0) Eq |= 1;
+                    const W D0n = (((Eq & pv) + pv) ^ pv) | Eq | mv | TR;
+                    W Ph = mv | ~(D0n | pv);
+                    W Mh = D0n & pv;
+                    const int top = (b == last_blk) ? last_bit : B - 1;
+                    const int hout = (int)((Ph >> top) & 1) - (int)((Mh >> top) & 1);
+                    Ph <<= 1; Mh <<= 1;
+                    if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
+                    Pv[b] = Mh | ~(D0n | Ph);
+                    Mv[b] = Ph & D0n;
+                    D0[b] = D0n;
+                    hin = hout;
+                }
+            }
+        }
+        return hin;
+    }
+};
+
+// One warp scores pattern `pat` against every to-string of its split.  LCS = false: Levenshtein, or with OSA = true optimal
+// string alignment (LevColumn); LCS = true: longest common subsequence (Hyyro 2004) -> Indel = la + lb - 2*LCS.
 // TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings.
 // (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; 0 = unspecified)
 template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false, bool OSA = false>
@@ -90,140 +185,52 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
     const int lane = lane_id();
     const int w = threadIdx.x >> 5;
     W *peq = reinterpret_cast<W *>(dyn) + (size_t)w * 256 * NW;              // peq[sym * NW + block]
-    const int split = blockIdx.y;
-    const int n_grp = (P.n_to + 31) >> 5;
-    const int per = (n_grp + P.n_splits - 1) / P.n_splits;
-    const int g_lo = split * per, g_hi = min(n_grp, g_lo + per);
-    int32_t *counter = P.counter + split;
 
     for (;;) {
-        int q = 0;
-        if (lane == 0) q = atomicAdd(counter, 1);
-        q = __shfl_sync(FULL, q, 0);
-        if (q >= P.n_ids) break;
-        const int i = P.from_ids[q];
+        const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
+        if (i < 0) break;
+        const GroupRange gr = split_groups(P.n_to, P.n_splits);    // per row: held across rows, ptxas spilled it (LCS, 8+ words)
         const int64_t fb = P.from_off[i];
         const int m = (int)(P.from_off[i + 1] - fb);
-        // match masks
-        for (int e = lane; e < 256 * NW; e += 32) peq[e] = 0;
-        __syncwarp();
-        for (int p = lane; p < m; p += 32) {
-            const uint32_t c = P.from_blob[fb + p];
-            const int s = c < 0x110000u ? P.sym_table[c] : 0;
-            if (s) {
-                if (sizeof(W) == 8) atomicOr(reinterpret_cast<unsigned long long *>(&peq[s * NW + p / B]), 1ull << (p % B));
-                else atomicOr(reinterpret_cast<unsigned *>(&peq[s * NW + p / B]), 1u << (p % B));
-            }
-        }
-        __syncwarp();
+        build_peq<W, NW>(peq, P.from_blob + fb, m, P.sym_table);
         const int last_bit = (m - 1) & (B - 1);          // bit of row m inside the last block (m > 0)
         const int last_blk = m > 0 ? (m - 1) / B : 0;
 
-        double best_s = 0.0; int best_j = -1, best_d = -1;
+        WarpArgBest<> best;
         WarpTopK top;
-        if constexpr (TOPK) top.init(P.k);
-        for (int g = g_lo; g < g_hi; ++g) {
+        if constexpr (TOPK) top.init(P.k); else best.init();
+        for (int g = gr.lo; g < gr.hi; ++g) {
             double cand_s = 0.0; int cand_j = -1;
             const int p = g * 32 + lane;
             const bool have = p < P.n_to;
             const int n = have ? P.slen[p] : 0;
             const int orig = have ? P.sorig[p] : -1;
-            int nmax = n;
-#pragma unroll
-            for (int d = 16; d; d >>= 1) nmax = max(nmax, __shfl_xor_sync(FULL, nmax, d));
             const uint32_t *src = P.packed + P.grp_word_off[g] + lane;
             int dist;
-            if (!LCS) {
-                W Pv[NW], Mv[NW];
-                W D0[NW], PMo[NW];                                    // OSA: D0 and Peq of the previous text symbol
-#pragma unroll
-                for (int b = 0; b < NW; ++b) {
-                    Pv[b] = ~(W)0; Mv[b] = 0;
-                    if constexpr (OSA) { D0[b] = 0; PMo[b] = 0; }     // PMo = 0: no transposition at the first symbol
-                }
+            if constexpr (!LCS) {
+                LevColumn<W, NW, OSA> col;
+                col.init();
                 int score = m;
-                uint32_t nextw = nmax > 0 ? src[0] : 0u;
-                for (int j0 = 0; j0 < nmax; j0 += 4) {
-                    const uint32_t word = nextw;
-                    if (j0 + 4 < nmax) nextw = src[(size_t)((j0 >> 2) + 1) * 32];      // prefetch: the recurrence below is a long dependent chain
-#pragma unroll
-                    for (int bb = 0; bb < 4; ++bb) {
-                        if (j0 + bb < n) {
-                            const int s = (word >> (8 * bb)) & 0xff;
-                            int hin = 1;                              // D[0][j] - D[0][j-1] = +1
-                            W trc = 0;                                // OSA: top bit of the block below's X
-#pragma unroll
-                            for (int b = 0; b < NW; ++b) {
-                                if (b <= last_blk) {
-                                    W Eq = peq[s * NW + b];
-                                    const W pv = Pv[b], mv = Mv[b];
-                                    if constexpr (!OSA) {
-                                        const W Xv = Eq | mv;
-                                        if (hin < 0) Eq |= 1;
-                                        const W Xh = (((Eq & pv) + pv) ^ pv) | Eq;
-                                        W Ph = mv | ~(Xh | pv);
-                                        W Mh = pv & Xh;
-                                        const int top = (b == last_blk) ? last_bit : B - 1;
-                                        const int hout = (int)((Ph >> top) & 1) - (int)((Mh >> top) & 1);
-                                        Ph <<= 1; Mh <<= 1;
-                                        if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
-                                        Pv[b] = Mh | ~(Xv | Ph);
-                                        Mv[b] = Ph & Xv;
-                                        hin = hout;
-                                    } else {
-                                        // X: rows that match this symbol where the previous column had no diagonal zero;
-                                        // one row up and ANDed with the previous symbol's matches, it marks a swap of b[j-1], b[j]
-                                        const W X = ~D0[b] & Eq;
-                                        const W TR = ((X << 1) | trc) & PMo[b];
-                                        trc = X >> (B - 1);
-                                        PMo[b] = Eq;
-                                        if (hin < 0) Eq |= 1;
-                                        const W D0n = (((Eq & pv) + pv) ^ pv) | Eq | mv | TR;
-                                        W Ph = mv | ~(D0n | pv);
-                                        W Mh = D0n & pv;
-                                        const int top = (b == last_blk) ? last_bit : B - 1;
-                                        const int hout = (int)((Ph >> top) & 1) - (int)((Mh >> top) & 1);
-                                        Ph <<= 1; Mh <<= 1;
-                                        if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
-                                        Pv[b] = Mh | ~(D0n | Ph);
-                                        Mv[b] = Ph & D0n;
-                                        D0[b] = D0n;
-                                        hin = hout;
-                                    }
-                                }
-                            }
-                            score += hin;                            // horizontal delta of row m
-                        }
-                    }
-                }
+                for_each_text_symbol(src, n, [&](int s) { score += col.step(peq + s * NW, last_blk, last_bit); });
                 dist = m > 0 ? score : n;
             } else {
                 W S[NW];
 #pragma unroll
                 for (int b = 0; b < NW; ++b) S[b] = ~(W)0;
-                uint32_t nextw = nmax > 0 ? src[0] : 0u;
-                for (int j0 = 0; j0 < nmax; j0 += 4) {
-                    const uint32_t word = nextw;
-                    if (j0 + 4 < nmax) nextw = src[(size_t)((j0 >> 2) + 1) * 32];
+                for_each_text_symbol(src, n, [&](int s) {
+                    unsigned carry = 0;
 #pragma unroll
-                    for (int bb = 0; bb < 4; ++bb) {
-                        if (j0 + bb < n) {
-                            const int s = (word >> (8 * bb)) & 0xff;
-                            unsigned carry = 0;
-#pragma unroll
-                            for (int b = 0; b < NW; ++b) {
-                                if (b <= last_blk) {
-                                    const W Eq = peq[s * NW + b];
-                                    const W x = S[b], u = x & Eq;
-                                    // S' = (S + (S & Eq)) | (S - (S & Eq)); u is a subset of x, so x - u = x & ~Eq (no borrow);
-                                    // the addition carries across blocks
-                                    const W sum = x + u; unsigned c1 = sum < x; const W sum2 = sum + carry; c1 |= (sum2 < sum); carry = c1;
-                                    S[b] = sum2 | (x & ~Eq);
-                                }
-                            }
+                    for (int b = 0; b < NW; ++b) {
+                        if (b <= last_blk) {
+                            const W Eq = peq[s * NW + b];
+                            const W x = S[b], u = x & Eq;
+                            // S' = (S + (S & Eq)) | (S - (S & Eq)); u is a subset of x, so x - u = x & ~Eq (no borrow);
+                            // the addition carries across blocks
+                            const W sum = x + u; unsigned c1 = sum < x; const W sum2 = sum + carry; c1 |= (sum2 < sum); carry = c1;
+                            S[b] = sum2 | (x & ~Eq);
                         }
                     }
-                }
+                });
                 int lcs = 0;
 #pragma unroll
                 for (int b = 0; b < NW; ++b) {
@@ -244,26 +251,11 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
                 if ((OSA ? P.metric == PFZ_METRIC_NORM_OSA : (P.metric == PFZ_METRIC_NORM_LEV || P.metric == PFZ_METRIC_RATIO)) &&
                     !(sc >= P.cutoff)) ok = false;
                 if constexpr (TOPK) { cand_s = sc; cand_j = ok ? orig : -1; }
-                else if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = dist; }
+                else if (ok) best.offer(sc, orig, dist);
             }
             if constexpr (TOPK) top.offer(cand_s, cand_j);
         }
-        if constexpr (TOPK) {
-            const size_t o = ((size_t)split * P.n_from + i) * P.k;
-            top.store(P.part_idx + o, P.part_score + o);
-        } else {
-            // first maximal score = lowest original index among the maxima
-#pragma unroll
-            for (int d = 16; d; d >>= 1) {
-                const double os = shfl_d(best_s, lane ^ d);
-                const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
-                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
-            }
-            if (lane == 0) {
-                const size_t o = (size_t)split * P.n_from + i;
-                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
-            }
-        }
+        store_row<TOPK>(P, i, top, best);
         __syncwarp();
     }
 }
@@ -297,37 +289,20 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
     W *peq = reinterpret_cast<W *>(dyn) + (size_t)w * 256 * NW;              // peq[sym * NW + block]
     uint8_t *store = dyn + (size_t)WARPS * 256 * NW * sizeof(W) + (size_t)w * STORE * 32 + lane;    // store[k * 32]
     const bool winkler = P.metric == PFZ_METRIC_JARO_WINKLER;
-    const int split = blockIdx.y;
-    const int n_grp = (P.n_to + 31) >> 5;
-    const int per = (n_grp + P.n_splits - 1) / P.n_splits;
-    const int g_lo = split * per, g_hi = min(n_grp, g_lo + per);
-    int32_t *counter = P.counter + split;
+    const GroupRange gr = split_groups(P.n_to, P.n_splits);
 
     for (;;) {
-        int q = 0;
-        if (lane == 0) q = atomicAdd(counter, 1);
-        q = __shfl_sync(FULL, q, 0);
-        if (q >= P.n_ids) break;
-        const int i = P.from_ids[q];
+        const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
+        if (i < 0) break;
         const int64_t fb = P.from_off[i];
         const int m = (int)(P.from_off[i + 1] - fb);
-        for (int e = lane; e < 256 * NW; e += 32) peq[e] = 0;
-        __syncwarp();
-        for (int p = lane; p < m; p += 32) {
-            const uint32_t c = P.from_blob[fb + p];
-            const int s = c < 0x110000u ? P.sym_table[c] : 0;
-            if (s) {
-                if (sizeof(W) == 8) atomicOr(reinterpret_cast<unsigned long long *>(&peq[s * NW + p / B]), 1ull << (p % B));
-                else atomicOr(reinterpret_cast<unsigned *>(&peq[s * NW + p / B]), 1u << (p % B));
-            }
-        }
-        __syncwarp();
+        build_peq<W, NW>(peq, P.from_blob + fb, m, P.sym_table);
         const int last_blk = m > 0 ? (m - 1) / B : 0;                          // blocks above it hold no pattern bits
 
-        double best_s = 0.0; int best_j = -1, best_d = -1;
+        WarpArgBest<> best;
         WarpTopK top;
-        if constexpr (TOPK) top.init(P.k);
-        for (int g = g_lo; g < g_hi; ++g) {
+        if constexpr (TOPK) top.init(P.k); else best.init();
+        for (int g = gr.lo; g < gr.hi; ++g) {
             double cand_s = 0.0; int cand_j = -1;
             const int p = g * 32 + lane;
             const bool have = p < P.n_to;
@@ -396,25 +371,11 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
             if (have) {
                 bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) && sc >= P.cutoff;
                 if constexpr (TOPK) { cand_s = sc; cand_j = ok ? orig : -1; }
-                else if (ok && (best_j < 0 || sc > best_s || (sc == best_s && orig < best_j))) { best_s = sc; best_j = orig; best_d = k; }
+                else if (ok) best.offer(sc, orig, k);
             }
             if constexpr (TOPK) top.offer(cand_s, cand_j);
         }
-        if constexpr (TOPK) {
-            const size_t o = ((size_t)split * P.n_from + i) * P.k;
-            top.store(P.part_idx + o, P.part_score + o);
-        } else {
-#pragma unroll
-            for (int d = 16; d; d >>= 1) {
-                const double os = shfl_d(best_s, lane ^ d);
-                const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
-                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
-            }
-            if (lane == 0) {
-                const size_t o = (size_t)split * P.n_from + i;
-                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
-            }
-        }
+        store_row<TOPK>(P, i, top, best);
         __syncwarp();
     }
 }
@@ -429,86 +390,10 @@ __global__ void lev_merge_kernel(const int32_t *__restrict__ part_idx, const dou
             const int j = part_idx[o];
             if (j < 0) continue;
             const double sc = part_score[o];
-            if (bj < 0 || sc > bs || (sc == bs && j < bj)) { bs = sc; bj = j; bd = part_dist[o]; }
+            if (bj < 0 || WarpTopK::before(sc, j, bs, bj)) { bs = sc; bj = j; bd = part_dist[o]; }
         }
         best_idx[i] = bj; best_score[i] = bj >= 0 ? bs : 0.0; best_dist[i] = bd;
     }
-}
-
-template <typename W, int NW, bool LCS, bool TOPK, bool OSA = false>
-static int launch_lev(const LevParams &P, int sms, cudaStream_t st) {
-    constexpr int WARPS = 4;
-    const size_t smem = (size_t)WARPS * 256 * NW * sizeof(W);
-    auto kernel = lev_kernel<W, NW, LCS, WARPS, TOPK, OSA>;
-    PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 0;
-    PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
-    if (occ < 1) occ = 1;
-    int gx = sms * occ;
-    const int need = (P.n_ids + WARPS - 1) / WARPS;
-    if (gx > need) gx = need;
-    if (gx < 1) gx = 1;
-    kernel<<<dim3(gx, P.n_splits), WARPS * 32, smem, st>>>(P);
-    PFZ_LAUNCH_OK();
-    return 0;
-}
-
-// Shared memory per warp: Peq (256 x NW words) plus the match store (32 lanes x B*NW bytes), the same size again.
-// Up to 64 KB per CTA: 4 warps up to 256 code points, 2 at 512, 1 at 1 024.
-template <typename W, int NW, bool TOPK>
-static int launch_jaro(const LevParams &P, int sms, cudaStream_t st) {
-    constexpr size_t PER_WARP = 2 * 256 * NW * sizeof(W);
-    constexpr int WARPS = PER_WARP * 4 <= 65536 ? 4 : PER_WARP * 2 <= 65536 ? 2 : 1;
-    const size_t smem = (size_t)WARPS * PER_WARP;
-    auto kernel = jaro_kernel<W, NW, WARPS, TOPK>;
-    PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 0;
-    PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
-    if (occ < 1) occ = 1;
-    int gx = sms * occ;
-    const int need = (P.n_ids + WARPS - 1) / WARPS;
-    if (gx > need) gx = need;
-    if (gx < 1) gx = 1;
-    kernel<<<dim3(gx, P.n_splits), WARPS * 32, smem, st>>>(P);
-    PFZ_LAUNCH_OK();
-    return 0;
-}
-
-// word class -> kernel instantiation (the metric picks Levenshtein, Indel, OSA or Jaro)
-template <bool TOPK>
-static int launch_class(const LevParams &P, int n_words, int sms, cudaStream_t st) {
-    if (P.metric == PFZ_METRIC_OSA || P.metric == PFZ_METRIC_NORM_OSA) {
-        switch (n_words) {
-            case 0: return launch_lev<uint32_t, 1, false, TOPK, true>(P, sms, st);
-            case 1: return launch_lev<uint64_t, 1, false, TOPK, true>(P, sms, st);
-            case 2: return launch_lev<uint64_t, 2, false, TOPK, true>(P, sms, st);
-            case 4: return launch_lev<uint64_t, 4, false, TOPK, true>(P, sms, st);
-            case 8: return launch_lev<uint64_t, 8, false, TOPK, true>(P, sms, st);
-            default: return launch_lev<uint64_t, 16, false, TOPK, true>(P, sms, st);
-        }
-    }
-    if (P.metric == PFZ_METRIC_JARO || P.metric == PFZ_METRIC_JARO_WINKLER) {
-        switch (n_words) {
-            case 0: return launch_jaro<uint32_t, 1, TOPK>(P, sms, st);
-            case 1: return launch_jaro<uint64_t, 1, TOPK>(P, sms, st);
-            case 2: return launch_jaro<uint64_t, 2, TOPK>(P, sms, st);
-            case 4: return launch_jaro<uint64_t, 4, TOPK>(P, sms, st);
-            case 8: return launch_jaro<uint64_t, 8, TOPK>(P, sms, st);
-            default: return launch_jaro<uint64_t, 16, TOPK>(P, sms, st);
-        }
-    }
-    const bool lcs = (P.metric == PFZ_METRIC_INDEL || P.metric == PFZ_METRIC_RATIO);
-#define PFZ_LEV_CASE(NWv, Wt)                                                            \
-    return lcs ? launch_lev<Wt, NWv, true, TOPK>(P, sms, st) : launch_lev<Wt, NWv, false, TOPK>(P, sms, st)
-    switch (n_words) {
-        case 0: PFZ_LEV_CASE(1, uint32_t);
-        case 1: PFZ_LEV_CASE(1, uint64_t);
-        case 2: PFZ_LEV_CASE(2, uint64_t);
-        case 4: PFZ_LEV_CASE(4, uint64_t);
-        case 8: PFZ_LEV_CASE(8, uint64_t);
-        default: PFZ_LEV_CASE(16, uint64_t);
-    }
-#undef PFZ_LEV_CASE
 }
 
 // ---- unrestricted Damerau-Levenshtein (DESIGN.md 4.10) ------------------------------------------------------------------
@@ -527,6 +412,7 @@ struct DlLayout {                       // one warp's shared memory
     static constexpr size_t STATE = (size_t)3 * (MAXM + 1) * 32 * sizeof(int16_t);      // A, P2, RK: [row][lane]
     static constexpr size_t PAT = (MAXM + 1 + 15) / 16 * 16;                            // pattern symbols, 1-based
     static constexpr size_t PER_WARP = PEQ + QUEUE + STATE + PAT;
+    static_assert(PER_WARP % 16 == 0 && PER_WARP <= 227 * 1024, "DL state does not fit one warp's shared memory");
 };
 
 // Exact unrestricted Damerau-Levenshtein (Lowrance-Wagner, unit costs) of pat[1..m] against the lane's text (n symbols in the
@@ -588,39 +474,21 @@ __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, co
     const bool norm = P.metric == PFZ_METRIC_NORM_DL;
     const bool full = P.matrix != nullptr;                                  // matrix mode: the DP on every pair
     const double NEG_INF = -CUDART_INF;
-    const int split = blockIdx.y;
-    const int n_grp = (P.n_to + 31) >> 5;
-    const int per = (n_grp + P.n_splits - 1) / P.n_splits;
-    const int g_lo = split * per, g_hi = min(n_grp, g_lo + per);
-    int32_t *counter = P.counter + split;
+    const GroupRange gr = split_groups(P.n_to, P.n_splits);
 
     for (;;) {
-        int q = 0;
-        if (lane == 0) q = atomicAdd(counter, 1);
-        q = __shfl_sync(FULL, q, 0);
-        if (q >= P.n_ids) break;
-        const int i = P.from_ids[q];
+        const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
+        if (i < 0) break;
         const int64_t fb = P.from_off[i];
         const int m = (int)(P.from_off[i + 1] - fb);
-        for (int e = lane; e < 256 * NW; e += 32) peq[e] = 0;
-        __syncwarp();
-        for (int p = lane; p < m; p += 32) {
-            const uint32_t c = P.from_blob[fb + p];
-            const int s = c < 0x110000u ? P.sym_table[c] : 0;
-            pat[p + 1] = (uint8_t)s;
-            if (s) {
-                if (sizeof(W) == 8) atomicOr(reinterpret_cast<unsigned long long *>(&peq[s * NW + p / B]), 1ull << (p % B));
-                else atomicOr(reinterpret_cast<unsigned *>(&peq[s * NW + p / B]), 1u << (p % B));
-            }
-        }
-        __syncwarp();
+        build_peq<W, NW>(peq, P.from_blob + fb, m, P.sym_table, pat);
         const int last_bit = (m - 1) & (B - 1);
         const int last_blk = m > 0 ? (m - 1) / B : 0;
         const double gt = gate ? gate[i] : NEG_INF;
 
-        double best_s = 0.0; int best_j = -1, best_d = -1;
+        WarpArgBest<> best;
         WarpTopK top;
-        if constexpr (TOPK) top.init(P.k);
+        if constexpr (TOPK) top.init(P.k); else best.init();
         double kth = NEG_INF;                                               // warp-uniform running k-th exact score
         int qn = 0;                                                         // warp-uniform queue fill
 
@@ -637,8 +505,8 @@ __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, co
                 const double ts = shfl_d(top.s, P.k - 1);
                 kth = __shfl_sync(FULL, top.j, P.k - 1) >= 0 ? ts : NEG_INF;
             } else {
-                if (cj >= 0 && (best_j < 0 || sc > best_s || (sc == best_s && cj < best_j))) { best_s = sc; best_j = cj; best_d = d; }
-                double v = best_j >= 0 ? best_s : NEG_INF;
+                best.offer(sc, cj, d);
+                double v = best.j >= 0 ? best.s : NEG_INF;
 #pragma unroll
                 for (int o = 16; o; o >>= 1) v = fmax(v, shfl_d(v, lane ^ o));
                 kth = v;
@@ -658,57 +526,16 @@ __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, co
             offer(run, d, n, orig);
         };
 
-        for (int g = g_lo; g < g_hi; ++g) {
+        for (int g = gr.lo; g < gr.hi; ++g) {
             const int p = g * 32 + lane;
             const bool have = p < P.n_to;
             const int n = have ? P.slen[p] : 0;
             const int orig = have ? P.sorig[p] : -1;
-            int nmax = n;
-#pragma unroll
-            for (int d = 16; d; d >>= 1) nmax = max(nmax, __shfl_xor_sync(FULL, nmax, d));
             const uint32_t *src = P.packed + P.grp_word_off[g] + lane;
-            // OSA, bit-parallel: lev_kernel's OSA recurrence (DESIGN.md 4.9)
-            W Pv[NW], Mv[NW], D0[NW], PMo[NW];
-#pragma unroll
-            for (int b = 0; b < NW; ++b) { Pv[b] = ~(W)0; Mv[b] = 0; D0[b] = 0; PMo[b] = 0; }
+            LevColumn<W, NW, true> col;
+            col.init();
             int score_m = m;
-            uint32_t nextw = nmax > 0 ? src[0] : 0u;
-            for (int j0 = 0; j0 < nmax; j0 += 4) {
-                const uint32_t word = nextw;
-                if (j0 + 4 < nmax) nextw = src[(size_t)((j0 >> 2) + 1) * 32];
-#pragma unroll
-                for (int bb = 0; bb < 4; ++bb) {
-                    if (j0 + bb < n) {
-                        const int s = (word >> (8 * bb)) & 0xff;
-                        int hin = 1;
-                        W trc = 0;
-#pragma unroll
-                        for (int b = 0; b < NW; ++b) {
-                            if (b <= last_blk) {
-                                W Eq = peq[s * NW + b];
-                                const W pv = Pv[b], mv = Mv[b];
-                                const W X = ~D0[b] & Eq;
-                                const W TR = ((X << 1) | trc) & PMo[b];
-                                trc = X >> (B - 1);
-                                PMo[b] = Eq;
-                                if (hin < 0) Eq |= 1;
-                                const W D0n = (((Eq & pv) + pv) ^ pv) | Eq | mv | TR;
-                                W Ph = mv | ~(D0n | pv);
-                                W Mh = D0n & pv;
-                                const int top_bit = (b == last_blk) ? last_bit : B - 1;
-                                const int hout = (int)((Ph >> top_bit) & 1) - (int)((Mh >> top_bit) & 1);
-                                Ph <<= 1; Mh <<= 1;
-                                if (hin < 0) Mh |= 1; else if (hin > 0) Ph |= 1;
-                                Pv[b] = Mh | ~(D0n | Ph);
-                                Mv[b] = Ph & D0n;
-                                D0[b] = D0n;
-                                hin = hout;
-                            }
-                        }
-                        score_m += hin;
-                    }
-                }
-            }
+            for_each_text_symbol(src, n, [&](int s) { score_m += col.step(peq + s * NW, last_blk, last_bit); });
             const int osa = m > 0 ? score_m : n;
             const int lb = max((2 * osa + 2) / 3, abs(m - n));
             const bool excl = P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift;
@@ -739,58 +566,76 @@ __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, co
         }
         if (qn > 0) flush(qn);
 
-        if constexpr (TOPK) {
-            const size_t o = ((size_t)split * P.n_from + i) * P.k;
-            top.store(P.part_idx + o, P.part_score + o);
-        } else {
-#pragma unroll
-            for (int d = 16; d; d >>= 1) {
-                const double os = shfl_d(best_s, lane ^ d);
-                const int oj = __shfl_xor_sync(FULL, best_j, d), od = __shfl_xor_sync(FULL, best_d, d);
-                if (oj >= 0 && (best_j < 0 || os > best_s || (os == best_s && oj < best_j))) { best_s = os; best_j = oj; best_d = od; }
-            }
-            if (lane == 0) {
-                const size_t o = (size_t)split * P.n_from + i;
-                P.part_idx[o] = best_j; P.part_score[o] = best_j >= 0 ? best_s : 0.0; P.part_dist[o] = best_d;
-            }
-        }
+        store_row<TOPK>(P, i, top, best);
         __syncwarp();
     }
 }
 
-// Shared memory per warp (DlLayout): 7.6 KB at 32 symbols, 15 KB at 64, ..., 225 KB at 1 024 -- 4 warps per CTA up to 128
-// symbols, 2 at 256, 1 from 512 on.
-template <typename W, int NW, bool TOPK>
-static int launch_dl(const LevParams &P, const double *gate, int sms, cudaStream_t st) {
-    using Lay = DlLayout<W, NW>;
-    constexpr size_t SMEM_MAX = 227 * 1024;
-    static_assert(Lay::PER_WARP % 16 == 0 && Lay::PER_WARP <= SMEM_MAX, "DL state does not fit one warp's shared memory");
-    constexpr int WARPS = Lay::PER_WARP * 4 <= SMEM_MAX ? 4 : Lay::PER_WARP * 2 <= SMEM_MAX ? 2 : 1;
-    const size_t smem = (size_t)WARPS * Lay::PER_WARP;
-    auto kernel = dl_kernel<W, NW, WARPS, TOPK>;
-    PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 0;
-    PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, WARPS * 32, smem));
-    if (occ < 1) occ = 1;
-    int gx = sms * occ;
-    const int need = (P.n_ids + WARPS - 1) / WARPS;
-    if (gx > need) gx = need;
-    if (gx < 1) gx = 1;
-    kernel<<<dim3(gx, P.n_splits), WARPS * 32, smem, st>>>(P, gate);
-    PFZ_LAUNCH_OK();
-    return 0;
+template <typename W, int NW> struct WordClass { using Word = W; static constexpr int N = NW; };
+
+// n_words (0: one 32-bit word; 1, 2, 4, 8, 16 64-bit words) -> f(WordClass<W, NW>())
+template <typename F>
+static int dispatch_words(int n_words, F &&f) {
+    switch (n_words) {
+        case 0: return f(WordClass<uint32_t, 1>());
+        case 1: return f(WordClass<uint64_t, 1>());
+        case 2: return f(WordClass<uint64_t, 2>());
+        case 4: return f(WordClass<uint64_t, 4>());
+        case 8: return f(WordClass<uint64_t, 8>());
+        default: return f(WordClass<uint64_t, 16>());
+    }
 }
 
+// word class -> kernel instantiation; the metric picks Levenshtein, Indel, OSA, Jaro or DL (gate: DL only)
 template <bool TOPK>
-static int launch_dl_class(const LevParams &P, const double *gate, int n_words, int sms, cudaStream_t st) {
-    switch (n_words) {
-        case 0: return launch_dl<uint32_t, 1, TOPK>(P, gate, sms, st);
-        case 1: return launch_dl<uint64_t, 1, TOPK>(P, gate, sms, st);
-        case 2: return launch_dl<uint64_t, 2, TOPK>(P, gate, sms, st);
-        case 4: return launch_dl<uint64_t, 4, TOPK>(P, gate, sms, st);
-        case 8: return launch_dl<uint64_t, 8, TOPK>(P, gate, sms, st);
-        default: return launch_dl<uint64_t, 16, TOPK>(P, gate, sms, st);
-    }
+static int launch_class(const LevParams &P, const double *gate, int n_words, int sms, cudaStream_t st) {
+    const int mt = P.metric;
+    return dispatch_words(n_words, [&](auto c) {
+        using W = typename decltype(c)::Word;
+        constexpr int NW = decltype(c)::N;
+        if (mt == PFZ_METRIC_DL || mt == PFZ_METRIC_NORM_DL) {
+            // Shared memory per warp (DlLayout): 7.6 KB at 32 symbols, 15 KB at 64, ..., 225 KB at 1 024 -- 4 warps per CTA up
+            // to 256 symbols, 2 at 512, 1 at 1 024.
+            constexpr size_t PER_WARP = DlLayout<W, NW>::PER_WARP;
+            constexpr int WARPS = warps_within(PER_WARP, 227 * 1024);
+            return launch_rows(dl_kernel<W, NW, WARPS, TOPK>, WARPS, WARPS * PER_WARP, P.n_ids, P.n_splits, sms, st, P, gate);
+        }
+        if (mt == PFZ_METRIC_JARO || mt == PFZ_METRIC_JARO_WINKLER) {
+            // Shared memory per warp: Peq (256 x NW words) plus the match store (32 lanes x B*NW bytes), the same size again.
+            // Up to 64 KB per CTA: 4 warps up to 256 code points, 2 at 512, 1 at 1 024.
+            constexpr size_t PER_WARP = 2 * 256 * NW * sizeof(W);
+            constexpr int WARPS = warps_within(PER_WARP, 65536);
+            return launch_rows(jaro_kernel<W, NW, WARPS, TOPK>, WARPS, WARPS * PER_WARP, P.n_ids, P.n_splits, sms, st, P);
+        }
+        constexpr int WARPS = 4;
+        const size_t smem = (size_t)WARPS * 256 * NW * sizeof(W);
+        if (mt == PFZ_METRIC_OSA || mt == PFZ_METRIC_NORM_OSA)
+            return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK, true>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+        if (mt == PFZ_METRIC_INDEL || mt == PFZ_METRIC_RATIO)
+            return launch_rows(lev_kernel<W, NW, true, WARPS, TOPK>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+        return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+    });
+}
+
+// The body of the four K3 entry points after their metric checks: the checks they share, the row counters and the launch.
+// fn names the entry point in error messages.
+template <bool TOPK>
+static int run_k3(const char *fn, const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                  int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off,
+                  const int32_t *slen, const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self,
+                  int64_t self_shift, int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, int32_t *part_dist,
+                  int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "%s: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", fn, n_words);
+    PFZ_REQUIRE(n_splits >= 1, "%s: n_splits < 1", fn);
+    PFZ_REQUIRE(!TOPK || (k >= 1 && k <= 32), "%s: k=%d unsupported (1..32)", fn, k);
+    if (n_ids <= 0 || n_to < 0) return 0;
+    cudaStream_t st = as_stream(stream);
+    int sms = 0;
+    if (start_rows(counter, n_splits, st, &sms)) return 1;
+    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
+                exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter, k};
+    return launch_class<TOPK>(P, gate, n_words, sms, st);
 }
 
 }  // namespace pfz
@@ -815,20 +660,11 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
                     int32_t n_splits, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
                     int32_t *counter, void *stream) {
     PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_OSA, "pfz_lev_argbest: unknown metric %d", metric);
-    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_lev_argbest: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
-    PFZ_REQUIRE(n_splits >= 1, "pfz_lev_argbest: n_splits < 1");
     const bool jaro = metric == PFZ_METRIC_JARO || metric == PFZ_METRIC_JARO_WINKLER;
     PFZ_REQUIRE(!(jaro && matrix), "pfz_lev_argbest: the distance matrix is not available for the Jaro metrics (matrix must be NULL)");
-    if (n_ids <= 0 || n_to < 0) return 0;
-    cudaStream_t st = as_stream(stream);
-    int dev = 0, sms = 0;
-    PFZ_CUDA_OK(cudaGetDevice(&dev));
-    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
-    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
-                exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter, 1};
-    return launch_class<false>(P, n_words, sms, st);
+    return run_k3<false>("pfz_lev_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
+                         slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, 1, part_idx, part_score, part_dist,
+                         matrix, matrix_ld, nullptr, counter, stream);
 }
 
 int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
@@ -837,19 +673,9 @@ int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
                  int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, int32_t *counter, void *stream) {
     PFZ_REQUIRE((metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER) || metric == PFZ_METRIC_NORM_OSA,
                 "pfz_lev_topk: metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA)", metric);
-    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_lev_topk: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
-    PFZ_REQUIRE(n_splits >= 1, "pfz_lev_topk: n_splits < 1");
-    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_lev_topk: k=%d unsupported (1..32)", k);
-    if (n_ids <= 0 || n_to < 0) return 0;
-    cudaStream_t st = as_stream(stream);
-    int dev = 0, sms = 0;
-    PFZ_CUDA_OK(cudaGetDevice(&dev));
-    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
-    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
-                exclude_self, self_shift, n_splits, part_idx, part_score, nullptr, nullptr, 0, n_from, counter, k};
-    return launch_class<true>(P, n_words, sms, st);
+    return run_k3<true>("pfz_lev_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
+                        slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, k, part_idx, part_score, nullptr,
+                        nullptr, 0, nullptr, counter, stream);
 }
 
 int pfz_dl_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
@@ -858,19 +684,10 @@ int pfz_dl_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32
                    int32_t n_splits, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
                    const double *gate, int32_t *counter, void *stream) {
     PFZ_REQUIRE(metric == PFZ_METRIC_DL || metric == PFZ_METRIC_NORM_DL, "pfz_dl_argbest: metric %d unsupported (DL, NORM_DL)", metric);
-    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_dl_argbest: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
-    PFZ_REQUIRE(n_splits >= 1, "pfz_dl_argbest: n_splits < 1");
     PFZ_REQUIRE(!(matrix && gate), "pfz_dl_argbest: the distance matrix needs every pair, so gate must be NULL with a matrix");
-    if (n_ids <= 0 || n_to < 0) return 0;
-    cudaStream_t st = as_stream(stream);
-    int dev = 0, sms = 0;
-    PFZ_CUDA_OK(cudaGetDevice(&dev));
-    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
-    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
-                exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter, 1};
-    return launch_dl_class<false>(P, gate, n_words, sms, st);
+    return run_k3<false>("pfz_dl_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
+                         slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, 1, part_idx, part_score, part_dist,
+                         matrix, matrix_ld, gate, counter, stream);
 }
 
 int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
@@ -878,19 +695,9 @@ int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t 
                 const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
                 int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, const double *gate, int32_t *counter, void *stream) {
     PFZ_REQUIRE(metric == PFZ_METRIC_NORM_DL, "pfz_dl_topk: metric %d unsupported (NORM_DL)", metric);
-    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_dl_topk: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
-    PFZ_REQUIRE(n_splits >= 1, "pfz_dl_topk: n_splits < 1");
-    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_dl_topk: k=%d unsupported (1..32)", k);
-    if (n_ids <= 0 || n_to < 0) return 0;
-    cudaStream_t st = as_stream(stream);
-    int dev = 0, sms = 0;
-    PFZ_CUDA_OK(cudaGetDevice(&dev));
-    PFZ_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PFZ_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(int32_t) * (size_t)n_splits, st));
-    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
-                exclude_self, self_shift, n_splits, part_idx, part_score, nullptr, nullptr, 0, n_from, counter, k};
-    return launch_dl_class<true>(P, gate, n_words, sms, st);
+    return run_k3<true>("pfz_dl_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
+                        slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, k, part_idx, part_score, nullptr,
+                        nullptr, 0, gate, counter, stream);
 }
 
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits, int32_t n_from,

@@ -68,6 +68,24 @@ def _alphabet_batches(blob, offsets):
     return batches
 
 
+def symbol_table(cps):
+    """Code point -> byte symbol: the distinct code points cps (ascending) get 1, 2, ... and every other code point 0."""
+    table = np.zeros(N_CODE_POINTS, dtype=np.uint8)
+    ok = cps < N_CODE_POINTS
+    table[cps[ok]] = np.arange(1, len(cps) + 1, dtype=np.uint8)[:int(ok.sum())]
+    return table
+
+
+def group_word_offsets(lens):
+    """First 32-bit word of each group of 32 strings (lens in layout order) in the packed to-side layout, and the total at
+    the end: a group holds ceil(its longest / 4) x 32 words."""
+    n = len(lens)
+    gmax = np.maximum.reduceat(lens, np.arange(0, n, 32)) if n else np.zeros(0, np.int64)
+    goff = np.zeros((n + 31) // 32 + 1, dtype=np.int64)
+    np.cumsum(((gmax + 3) // 4) * 32, out=goff[1:])
+    return goff
+
+
 def _blob_to_dev(b):
     if b.size == 0:
         return torch.zeros(1, dtype=torch.int32, device=_dev())
@@ -96,10 +114,7 @@ class EditQueries:
         classes = np.select([lens <= 32, lens <= 64, lens <= 128, lens <= 256, lens <= 512], [0, 1, 2, 4, 8], 16).astype(np.int32)
         self.batches = []                                   # [(d_table, [(n_words, d_ids, n_ids), ...])]
         for lo, hi in _alphabet_batches(blob, off):
-            cps = np.unique(blob[off[lo]:off[hi]]).astype(np.int64)
-            table = np.zeros(N_CODE_POINTS, dtype=np.uint8)
-            ok = cps < N_CODE_POINTS
-            table[cps[ok]] = np.arange(1, len(cps) + 1, dtype=np.uint8)[:int(ok.sum())]
+            table = symbol_table(np.unique(blob[off[lo]:off[hi]]).astype(np.int64))
             groups = []
             for nw in (0, 1, 2, 4, 8, 16):
                 ids = np.nonzero(classes[lo:hi] == nw)[0].astype(np.int32) + lo
@@ -128,9 +143,7 @@ class EditTargets:
         self.lens = tlens
         order = np.argsort(tlens, kind="stable").astype(np.int32)
         self.n_grp = (self.n + 31) // 32
-        gmax = tlens[order[np.minimum(np.arange(self.n_grp) * 32 + 31, self.n - 1)]]
-        gwords = ((gmax + 3) // 4) * 32
-        goff = np.zeros(self.n_grp + 1, dtype=np.int64); np.cumsum(gwords, out=goff[1:])
+        goff = group_word_offsets(tlens[order])
         self.d_order = _to_dev(order); self.d_goff = _to_dev(goff)
         self.h2d_bytes += order.nbytes + goff.nbytes
         self.packed = torch.empty(max(int(goff[-1]), 1), dtype=torch.int32, device=dev)
@@ -141,6 +154,23 @@ def default_splits(n_from, n_grp):
     # ~4 (pattern, to-split) tasks per resident warp: patterns differ in length, finer tasks balance the tail
     want = 4 * 132 * 48
     return max(1, min(n_grp, (want + max(n_from, 1) - 1) // max(n_from, 1)))
+
+
+def _word_classes(Q, T):
+    """Per alphabet batch of Q: pack T under the batch's symbol table (pfz_lev_pack), then yield one
+    (d_table, n_words, d_ids, n_ids) per word class of the batch."""
+    for d_table, groups in Q.batches:
+        _lib.call("pfz_lev_pack", _p(T.d_blob), _p(T.d_off), _p(T.d_order), T.n, _p(d_table), _p(T.d_goff), _p(T.packed), _p(T.slen),
+                  _stream())
+        for nw, d_ids, n_ids in groups:
+            yield d_table, nw, d_ids, n_ids
+
+
+def _k3_head(Q, T, cls, metric, score_cutoff, exclude_self, self_shift, n_splits):
+    """The leading arguments of pfz_lev_argbest, pfz_lev_topk, pfz_dl_argbest and pfz_dl_topk (from_blob .. n_splits)."""
+    d_table, nw, d_ids, n_ids = cls
+    return (_p(Q.d_blob), _p(Q.d_off), Q.n, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff), _p(T.slen),
+            _p(T.d_order), T.n, METRIC[metric], float(score_cutoff), int(bool(exclude_self)), int(self_shift), n_splits)
 
 
 def _gate_fill(metric, score_cutoff):
@@ -172,29 +202,21 @@ def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=Fal
     part_score = torch.zeros((n_splits, n_from), dtype=torch.float64, device=dev)
     part_dist = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
     counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
-    dl = metric in DL_GATE
-    for d_table, groups in Q.batches:
-        _lib.call("pfz_lev_pack", _p(T.d_blob), _p(T.d_off), _p(T.d_order), n_to, _p(d_table), _p(T.d_goff), _p(T.packed), _p(T.slen), _stream())
-        for nw, d_ids, n_ids in groups:
-            if dl:
-                gate = None
-                if dl_gate and not want_matrix:
-                    _lib.call("pfz_lev_argbest", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
-                              _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[DL_GATE[metric]], float(score_cutoff),
-                              int(bool(exclude_self)), int(self_shift), n_splits, _p(part_idx), _p(part_score), _p(part_dist), None, 0,
-                              _p(counter), _stream())
-                    _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx),
-                              _p(best_score), _p(best_dist), _stream())
-                    gate = torch.where(best_idx >= 0, best_score, _gate_fill(metric, score_cutoff))
-                _lib.call("pfz_dl_argbest", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
-                          _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)),
-                          int(self_shift), n_splits, _p(part_idx), _p(part_score), _p(part_dist), _p(matrix),
-                          int(matrix.stride(0)) if matrix is not None else 0, _p(gate), _p(counter), _stream())
-                continue
-            _lib.call("pfz_lev_argbest", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
-                      _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)),
-                      int(self_shift), n_splits, _p(part_idx), _p(part_score), _p(part_dist), _p(matrix),
-                      int(matrix.stride(0)) if matrix is not None else 0, _p(counter), _stream())
+    mat = (_p(matrix), int(matrix.stride(0)) if matrix is not None else 0)
+    for cls in _word_classes(Q, T):
+        head = lambda m: _k3_head(Q, T, cls, m, score_cutoff, exclude_self, self_shift, n_splits)  # noqa: E731
+        if metric not in DL_GATE:
+            _lib.call("pfz_lev_argbest", *head(metric), _p(part_idx), _p(part_score), _p(part_dist), *mat, _p(counter), _stream())
+            continue
+        gate = None
+        if dl_gate and not want_matrix:
+            _lib.call("pfz_lev_argbest", *head(DL_GATE[metric]), _p(part_idx), _p(part_score), _p(part_dist), None, 0, _p(counter),
+                      _stream())
+            _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx),
+                      _p(best_score), _p(best_dist), _stream())
+            gate = torch.where(best_idx >= 0, best_score, _gate_fill(metric, score_cutoff))
+        _lib.call("pfz_dl_argbest", *head(metric), _p(part_idx), _p(part_score), _p(part_dist), *mat, _p(gate), _p(counter),
+                  _stream())
     _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx), _p(best_score),
               _p(best_dist), _stream())
     if to_index_base:
@@ -243,24 +265,17 @@ def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=Fal
     part_idx = torch.full((n_splits, n_from, k), -1, dtype=torch.int32, device=dev)
     part_score = torch.zeros((n_splits, n_from, k), dtype=torch.float64, device=dev)
     counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
-    for d_table, groups in Q.batches:
-        _lib.call("pfz_lev_pack", _p(T.d_blob), _p(T.d_off), _p(T.d_order), n_to, _p(d_table), _p(T.d_goff), _p(T.packed), _p(T.slen), _stream())
-        for nw, d_ids, n_ids in groups:
-            if metric in DL_GATE:
-                gate = None
-                if dl_gate:
-                    _lib.call("pfz_lev_topk", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed),
-                              _p(T.d_goff), _p(T.slen), _p(T.d_order), n_to, METRIC[DL_GATE[metric]], float(score_cutoff),
-                              int(bool(exclude_self)), int(self_shift), n_splits, k, _p(part_idx), _p(part_score), _p(counter), _stream())
-                    gi, gs = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
-                    gate = torch.where(gi[:, k - 1] >= 0, gs[:, k - 1], _gate_fill(metric, score_cutoff)).contiguous()
-                _lib.call("pfz_dl_topk", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
-                          _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)), int(self_shift),
-                          n_splits, k, _p(part_idx), _p(part_score), _p(gate), _p(counter), _stream())
-                continue
-            _lib.call("pfz_lev_topk", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
-                      _p(T.slen), _p(T.d_order), n_to, METRIC[metric], float(score_cutoff), int(bool(exclude_self)), int(self_shift),
-                      n_splits, k, _p(part_idx), _p(part_score), _p(counter), _stream())
+    for cls in _word_classes(Q, T):
+        head = lambda m: _k3_head(Q, T, cls, m, score_cutoff, exclude_self, self_shift, n_splits)  # noqa: E731
+        if metric not in DL_GATE:
+            _lib.call("pfz_lev_topk", *head(metric), k, _p(part_idx), _p(part_score), _p(counter), _stream())
+            continue
+        gate = None
+        if dl_gate:
+            _lib.call("pfz_lev_topk", *head(DL_GATE[metric]), k, _p(part_idx), _p(part_score), _p(counter), _stream())
+            gi, gs = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
+            gate = torch.where(gi[:, k - 1] >= 0, gs[:, k - 1], _gate_fill(metric, score_cutoff)).contiguous()
+        _lib.call("pfz_dl_topk", *head(metric), k, _p(part_idx), _p(part_score), _p(gate), _p(counter), _stream())
     idx, score = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
     if to_index_base:
         idx = torch.where(idx >= 0, idx + int(to_index_base), idx)

@@ -14,7 +14,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .editdist import N_CODE_POINTS, _alphabet_batches, _blob_to_dev, check_top_n, default_splits
+from .editdist import _alphabet_batches, _blob_to_dev, check_top_n, default_splits, group_word_offsets, symbol_table
 from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
@@ -91,10 +91,7 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
     d_order = _to_dev(order)
     packs = []
     for v in range(3):
-        lv = T.lens[v][order]
-        gmax = np.maximum.reduceat(lv, np.arange(0, n_to, 32)) if n_to else np.zeros(0, np.int64)
-        gwords = ((gmax + 3) // 4) * 32
-        goff = np.zeros(n_grp + 1, dtype=np.int64); np.cumsum(gwords, out=goff[1:])
+        goff = group_word_offsets(T.lens[v][order])
         packs.append((torch.empty(max(int(goff[-1]), 1), dtype=torch.int32, device=dev), _to_dev(goff),
                       torch.empty(n_to, dtype=torch.int32, device=dev)))
     if n_splits is None:
@@ -112,10 +109,7 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
         cps = np.unique(np.concatenate([fblob[foff[lo]:foff[hi]].astype(np.int64), np.array([0x20], dtype=np.int64)]))
         if len(cps) > 255:
             raise ValueError("a batch of from-strings has more than 254 distinct code points besides the space")
-        table = np.zeros(N_CODE_POINTS, dtype=np.uint8)
-        ok = cps < N_CODE_POINTS
-        table[cps[ok]] = np.arange(1, len(cps) + 1, dtype=np.uint8)[:int(ok.sum())]
-        d_table = _to_dev(table); keep.append(d_table)
+        d_table = _to_dev(symbol_table(cps)); keep.append(d_table)
         for v in range(3):
             _lib.call("pfz_lev_pack", _p(T.dev[v][0]), _p(T.dev[v][1]), _p(d_order), n_to, _p(d_table), _p(packs[v][1]), _p(packs[v][0]),
                       _p(packs[v][2]), _stream())
