@@ -296,8 +296,9 @@ int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t 
  * ptrs: 38 device pointers -- for the from-side then the to-side: {blob uint32, offsets int64} of s, S(s) = sorted tokens
  *       joined, U(s) = distinct sorted tokens joined; tok_ptr int32[n+1]; tok_ids int32 (distinct token ids per string,
  *       ascending; ids number the tokens of both lists in sorted order); sig uint64[n] (Bloom signature of the ids);
- *       n_tok_all int32[n] (tokens incl. duplicates) -- then from_ids int32[n_ids] (from-rows of this word class: n_words = 1, 2, 4
- *       for patterns up to 64, 128, 255 code points), sym_table uint8[0x110000], for each variant {packed, grp_word_off, slen}
+ *       n_tok_all int32[n] (tokens incl. duplicates) -- then from_ids int32[n_ids] (from-rows of this word class: n_words = 1, 2, 4,
+ *       8, 16 for from-strings whose longest variant has up to 64, 128, 256, 512, 1024 code points; to-strings of any
+ *       length), sym_table uint8[0x110000], for each variant {packed, grp_word_off, slen}
  *       (pfz_lev_pack layouts of b, S(b), U(b) in ONE length order), sorig int32[n_to], tok_blob uint32, tok_off int64[n_tok+1],
  *       part_idx int32[n_splits][n_from], part_score float64[n_splits][n_from], counter int32[n_splits], reserved (NULL).
  * Best = first to-string (lowest index) with the maximal score >= score_cutoff; merge the splits with pfz_lev_merge.          */

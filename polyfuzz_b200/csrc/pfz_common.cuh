@@ -1,5 +1,6 @@
 // pfz_common.cuh -- shared helpers for libpfz.so (sm_90a only), among them the row driver of K3 and K3b: split_groups,
-// claim_row, build_peq, the WarpTopK / WarpArgBest epilogues, start_rows and launch_rows.
+// claim_row (claim_row_cta and merge_cta for one CTA per row), build_peq, the WarpTopK / WarpArgBest epilogues, start_rows and
+// launch_rows / launch_ctas.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -131,14 +132,42 @@ __device__ __forceinline__ int claim_row(int32_t *counter, const int32_t *from_i
     return q < n_ids ? from_ids[q] : -1;
 }
 
-// One warp's match masks: peq[sym * NW + block] bit p is set where pattern symbol p is sym.  cps: the m code points, mapped by
-// sym_table (symbol 0, the text-only code points, matches nothing); pat (optional) receives the symbols 1-based.
-template <typename W, int NW>
+// ---- CTA-per-row variant (K3b's 8- and 16-word classes): the CTA's warps share one from-row and its match masks, and warp w
+// takes the split's to-groups lo + w, lo + w + warps, ...
+// the CTA's next from-row, or -1; the leading barrier keeps the previous row's shared state (masks, slot, merge buffers) alive
+// until every warp is done with it
+__device__ __forceinline__ int claim_row_cta(int32_t *counter, const int32_t *from_ids, int n_ids, int *slot) {
+    __syncthreads();
+    if (threadIdx.x == 0) *slot = atomicAdd(counter, 1);
+    __syncthreads();
+    const int q = *slot;
+    return q < n_ids ? from_ids[q] : -1;
+}
+
+// Merge the warps' WarpArgBest<false> or WarpTopK epilogues of one row: every lane leaves its (s, j) in sh_s / sh_j
+// [warps * 32], and warp 0 offers the other warps' entries lane by lane to its own epilogue.  Both keys are strict total
+// orders over distinct indices, so the result is that of one warp offered everything.  Returns true in warp 0, which then
+// stores the row's slot(s) as the one-warp layout does.
+template <typename Epi>
+__device__ __forceinline__ bool merge_cta(Epi &e, double *sh_s, int *sh_j) {
+    const int lane = lane_id(), w = threadIdx.x >> 5;
+    sh_s[threadIdx.x] = e.s; sh_j[threadIdx.x] = e.j;
+    __syncthreads();
+    if (w != 0) return false;
+    for (int v = 1; v < (int)(blockDim.x >> 5); ++v) e.offer(sh_s[v * 32 + lane], sh_j[v * 32 + lane]);
+    return true;
+}
+
+// One warp's (CTA = false) or the whole CTA's (CTA = true) match masks: peq[sym * NW + block] bit p is set where pattern symbol
+// p is sym.  cps: the m code points, mapped by sym_table (symbol 0, the text-only code points, matches nothing); pat (optional)
+// receives the symbols 1-based.
+template <typename W, int NW, bool CTA = false>
 __device__ __forceinline__ void build_peq(W *peq, const uint32_t *cps, int m, const uint8_t *sym_table, uint8_t *pat = nullptr) {
     constexpr int B = 8 * sizeof(W);
-    for (int e = lane_id(); e < 256 * NW; e += 32) peq[e] = 0;
-    __syncwarp();
-    for (int p = lane_id(); p < m; p += 32) {
+    const int t0 = CTA ? (int)threadIdx.x : lane_id(), nt = CTA ? (int)blockDim.x : 32;
+    for (int e = t0; e < 256 * NW; e += nt) peq[e] = 0;
+    if constexpr (CTA) __syncthreads(); else __syncwarp();
+    for (int p = t0; p < m; p += nt) {
         const uint32_t c = cps[p];
         const int s = c < 0x110000u ? sym_table[c] : 0;
         if (pat) pat[p + 1] = (uint8_t)s;
@@ -147,7 +176,7 @@ __device__ __forceinline__ void build_peq(W *peq, const uint32_t *cps, int m, co
             else atomicOr(reinterpret_cast<unsigned *>(&peq[s * NW + p / B]), 1u << (p % B));
         }
     }
-    __syncwarp();
+    if constexpr (CTA) __syncthreads(); else __syncwarp();
 }
 
 // warps per CTA (4, 2 or 1) for a kernel whose warps each take per_warp bytes of shared memory, within budget bytes per CTA
@@ -163,20 +192,24 @@ static inline int start_rows(int32_t *counter, int n_splits, cudaStream_t st, in
 }
 
 // Launch a row-driver kernel on (gx, n_splits) CTAs of `warps` warps: as many CTAs per split as fit the SMs at once, and no
-// more than n_ids rows need.
+// more than max_ctas (the CTAs the rows can keep busy).
 template <typename Kernel, typename... Args>
-static int launch_rows(Kernel kernel, int warps, size_t smem, int n_ids, int n_splits, int sms, cudaStream_t st, const Args &...args) {
+static int launch_ctas(Kernel kernel, int warps, size_t smem, int max_ctas, int n_splits, int sms, cudaStream_t st, const Args &...args) {
     PFZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     PFZ_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, warps * 32, smem));
     if (occ < 1) occ = 1;
     int gx = sms * occ;
-    const int need = (n_ids + warps - 1) / warps;
-    if (gx > need) gx = need;
+    if (gx > max_ctas) gx = max_ctas;
     if (gx < 1) gx = 1;
     kernel<<<dim3(gx, n_splits), warps * 32, smem, st>>>(args...);
     PFZ_LAUNCH_OK();
     return 0;
+}
+// one warp per row: n_ids rows keep (n_ids + warps - 1) / warps CTAs busy
+template <typename Kernel, typename... Args>
+static int launch_rows(Kernel kernel, int warps, size_t smem, int n_ids, int n_splits, int sms, cudaStream_t st, const Args &...args) {
+    return launch_ctas(kernel, warps, smem, (n_ids + warps - 1) / warps, n_splits, sms, st, args...);
 }
 
 // exclusive scan of int32 -> int32 on a stream; ws from pfz_scan_ws_bytes(n)

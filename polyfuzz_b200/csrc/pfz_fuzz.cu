@@ -16,18 +16,22 @@
 //   token_sort_ratio     LCS(S(a), S(b))
 //   token_set_ratio      token-id sets (sorted ids per string, 64-bit Bloom signature as a pre-filter): no common token ->
 //                        LCS(U(a), U(b)); a common token and one side a subset -> 100; else the differences are joined per
-//                        pair and scored by a small dynamic programme in local memory
+//                        pair and scored by a masked LCS over U(a)'s bits (fz_diff_indel)
 //   partial_ratio        the shorter string against every window of the longer one (prefixes shorter than it, all windows of
 //                        its length, suffixes): windows of the to-string restart the recurrence at the window start; windows of
 //                        the from-string mask Peq to the window's bits; prefix windows fall out of ONE pass (the number of zero
 //                        bits among the first i rows is LCS(a[:i], b))
 //   WRatio               the weighted combination (0.95 / 0.9 / 0.6, length-ratio switches 1.5 and 8) of the above.
 // Symbols are bytes (the host maps the code points of the from-list to 1..255, everything else to 0 = matches nothing).
+//
+// Word classes: NW = 1, 2, 4 (from-strings up to 256 code points) run one warp per from-row, WARPS warps per CTA, each warp
+// with its own masks of the three variants.  NW = 8, 16 (257..1 024) run one CTA per from-row (CTA_ROW): the CTA's warps share
+// the masks of the variants the scorer reads and take the split's to-groups in turn; their epilogues are merged at the end of
+// the row (merge_cta).  To-strings may have any length.
 #include "pfz_common.cuh"
 
 namespace pfz {
 
-constexpr int FZ_MAXLEN = 255;          // code points per string for these scorers (the host checks)
 enum { FZ_RATIO = 0, FZ_QRATIO = 1, FZ_PARTIAL = 2, FZ_TSORT = 3, FZ_TSET = 4, FZ_TRATIO = 5, FZ_PTSORT = 6, FZ_PTSET = 7, FZ_PTRATIO = 8, FZ_WRATIO = 9 };
 
 struct FuzzSide {                       // one string list with its derived variants (device pointers)
@@ -114,8 +118,10 @@ __device__ int fz_lcs(const uint64_t *__restrict__ peq, int m, const TextRef &t)
     return bp.zeros(0, m);
 }
 
-// best normalised Indel similarity of partial_ratio(pattern, text): rapidfuzz's window set (see the file header)
-template <int NW>
+// best normalised Indel similarity of partial_ratio(pattern, text): rapidfuzz's window set (see the file header).
+// SKIP (the long classes): a window whose boundary symbol -- the last one of a full window, the first one of a suffix -- does
+// not occur in the other string is not scored.  It is dominated by a scored neighbour (DESIGN §4.3), so the best is unchanged.
+template <int NW, bool SKIP = false>
 __device__ double fz_partial_best(const uint64_t *__restrict__ peq, int la, const TextRef &t) {
     const int lb = t.n;
     double best = 0.0;
@@ -129,6 +135,13 @@ __device__ double fz_partial_best(const uint64_t *__restrict__ peq, int la, cons
         }
         for (int i = 0; i < ll; ++i) {                     // windows text[i : i+ls] (i < ll-ls) and suffixes text[i:] (i >= ll-ls)
             const int e = min(ll, i + ls);
+            if constexpr (SKIP) {
+                const int s = text_sym(t, i < ll - ls ? e - 1 : i);
+                uint64_t any = 0;
+#pragma unroll
+                for (int b = 0; b < NW; ++b) any |= peq[s * NW + b];
+                if (!any) continue;
+            }
             bp.init();
             for (int j = i; j < e; ++j) bp.step(peq, text_sym(t, j), nullptr);
             best = fmax(best, fz_norm_sim(ls + (e - i) - 2 * bp.zeros(0, ls), ls + (e - i)));
@@ -137,11 +150,30 @@ __device__ double fz_partial_best(const uint64_t *__restrict__ peq, int la, cons
     if (la > lb || (la == lb && best != 1.0)) {            // shorter = text; windows of the pattern
         const int ls = lb, ll = la;
         Bp<NW> bp; bp.init();
-        for (int j = 0; j < ls; ++j) bp.step(peq, text_sym(t, j), nullptr);
+        uint64_t hit[SKIP ? NW : 1];                       // SKIP: the pattern rows whose symbol occurs in the text
+        if constexpr (SKIP) {
+#pragma unroll
+            for (int b = 0; b < NW; ++b) hit[b] = 0;
+        }
+        for (int j = 0; j < ls; ++j) {
+            const int s = text_sym(t, j);
+            bp.step(peq, s, nullptr);
+            if constexpr (SKIP) {
+#pragma unroll
+                for (int b = 0; b < NW; ++b) hit[b] |= peq[s * NW + b];
+            }
+        }
         for (int i = 1; i < ls; ++i)                       // prefixes pattern[:i]: rows 0..i-1 of the final state
             best = fmax(best, fz_norm_sim(ls + i - 2 * bp.zeros(0, i), ls + i));
         for (int i = 0; i < ll; ++i) {                     // windows pattern[i : i+ls] and suffixes pattern[i:]
             const int e = min(ll, i + ls);
+            if constexpr (SKIP) {
+                const int r = i < ll - ls ? e - 1 : i;
+                uint64_t hw = 0;
+#pragma unroll
+                for (int b = 0; b < NW; ++b) hw = b == (r >> 6) ? hit[b] : hw;
+                if (!((hw >> (r & 63)) & 1ull)) continue;
+            }
             uint64_t mask[NW];
 #pragma unroll
             for (int b = 0; b < NW; ++b) {
@@ -173,59 +205,87 @@ __device__ TokInfo fz_tok_info(const int32_t *a, int na, const int32_t *b, int n
     r.ba_len = ba + max(r.n_ba - 1, 0);
     return r;
 }
-// Indel distance of the joined differences (tokens of a not in b, sorted | tokens of b not in a, sorted): textbook LCS rows in
-// local memory; token ids ascend in the lists but the JOIN order is the lexicographic order of the token texts, which is the id
-// order by construction (the host numbers the tokens in sorted order)
-__device__ int fz_diff_indel(const int32_t *a, int na, const int32_t *b, int nb, const uint32_t *__restrict__ tok_blob,
-                             const int64_t *__restrict__ tok_off) {
-    uint32_t sa[FZ_MAXLEN + 1], sb[FZ_MAXLEN + 1];
-    uint8_t row[FZ_MAXLEN + 2];
-    int la = 0, lb = 0;
-    {
-        int p = 0, q = 0;
-        while (p < na || q < nb) {
-            const int x = p < na ? a[p] : 0x7fffffff, y = q < nb ? b[q] : 0x7fffffff;
-            if (x == y) { ++p; ++q; }
-            else if (x < y) {
-                if (la) sa[la++] = 0x20u;
-                for (int64_t c = tok_off[x]; c < tok_off[x + 1] && la <= FZ_MAXLEN; ++c) sa[la++] = tok_blob[c];
-                ++p;
-            } else {
-                if (lb) sb[lb++] = 0x20u;
-                for (int64_t c = tok_off[y]; c < tok_off[y + 1] && lb <= FZ_MAXLEN; ++c) sb[lb++] = tok_blob[c];
-                ++q;
+// Indel distance of the joined differences (tokens of a not in b, sorted | tokens of b not in a, sorted) as a bit-parallel LCS
+// over U(a)'s masks.  U(a) is a's distinct tokens in id order (= sorted order: the host numbers the tokens in sorted order)
+// joined by single spaces, so the from-side difference is the subsequence of U(a) made of its kept tokens and the space
+// before every kept token but the first.  The other rows are masked off: they never match, so the LCS against them is the
+// LCS against the difference.  The to-side difference is streamed from tok_blob (with its spaces) as the text; a code point
+// outside the alphabet maps to 0 and matches nothing.  No per-thread arrays; the text has any length.
+__device__ __forceinline__ int fz_sym(uint32_t c, const uint8_t *__restrict__ sym_table) { return c < 0x110000u ? sym_table[c] : 0; }
+
+template <int NW>
+__device__ int fz_diff_indel(const uint64_t *__restrict__ peq_u, const int32_t *a, int na, const int32_t *b, int nb,
+                             const uint32_t *__restrict__ tok_blob, const int64_t *__restrict__ tok_off, const uint8_t *__restrict__ sym_table) {
+    uint64_t mask[NW];
+#pragma unroll
+    for (int w = 0; w < NW; ++w) mask[w] = 0;
+    int la = 0;
+    for (int p = 0, q = 0, pos = 0; p < na; ++p) {         // a \ b: rows of U(a) kept
+        const int x = a[p];
+        while (q < nb && b[q] < x) ++q;
+        const int len = (int)(tok_off[x + 1] - tok_off[x]);
+        if (q >= nb || b[q] != x) {
+            const int l = la ? pos - 1 : pos, h = pos + len;
+            la += h - l;
+#pragma unroll
+            for (int w = 0; w < NW; ++w) {
+                const int lo = max(l - 64 * w, 0), hi = min(h - 64 * w, 64);
+                if (hi > lo) mask[w] |= (hi == 64 ? ~0ull : ((1ull << hi) - 1ull)) & ~((1ull << lo) - 1ull);
             }
         }
+        pos += len + 1;
     }
-    for (int j = 0; j <= lb; ++j) row[j] = 0;
-    for (int i = 1; i <= la; ++i) {
-        int diag = 0;
-        const uint32_t ca = sa[i - 1];
-        for (int j = 1; j <= lb; ++j) {
-            const int up = row[j];
-            const int bestv = (ca == sb[j - 1]) ? diag + 1 : max(up, (int)row[j - 1]);
-            diag = up;
-            row[j] = (uint8_t)bestv;
-        }
+    const int space = sym_table[0x20];
+    Bp<NW> bp; bp.init();
+    int lb = 0;
+    for (int p = 0, q = 0; q < nb; ++q) {                  // b \ a, streamed
+        const int y = b[q];
+        while (p < na && a[p] < y) ++p;
+        if (p < na && a[p] == y) continue;
+        if (lb) { bp.step(peq_u, space, mask); ++lb; }
+        for (int64_t c = tok_off[y]; c < tok_off[y + 1]; ++c, ++lb) bp.step(peq_u, fz_sym(tok_blob[c], sym_table), mask);
     }
-    return la + lb - 2 * (int)row[lb];
+    return la + lb - 2 * bp.zeros(0, 64 * NW);
 }
 
 // TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings
 // (the group's body is a do/while(0), so a lane that skips its pair still reaches the warp-wide offer).
-// (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; 0 = unspecified)
+// (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; for the arg-best
+// classes at 1 and 2 words, the blocks per SM their shared memory and registers allow, which keeps ptxas from spilling more)
+// CTA_ROW (NW >= 8): dyn holds the masks of the variants the scorer reads (fz_variants), in variant order, then the merge
+// buffers and the row slot (fz_cta_smem).
+__host__ __device__ constexpr bool fz_reads_plain(int sc) { return sc == FZ_RATIO || sc == FZ_QRATIO || sc == FZ_PARTIAL || sc == FZ_WRATIO; }
+__host__ __device__ constexpr bool fz_reads_sorted(int sc) { return sc == FZ_TSORT || sc == FZ_TRATIO || sc == FZ_PTSORT || sc == FZ_PTRATIO || sc == FZ_WRATIO; }
+__host__ __device__ constexpr bool fz_reads_uniq(int sc) { return sc == FZ_TSET || sc == FZ_TRATIO || sc == FZ_PTSET || sc == FZ_PTRATIO || sc == FZ_WRATIO; }
+__host__ __device__ constexpr int fz_variants(int sc) { return (int)fz_reads_plain(sc) + (int)fz_reads_sorted(sc) + (int)fz_reads_uniq(sc); }
+constexpr size_t fz_cta_smem(int nw, int warps, int sc) { return (size_t)fz_variants(sc) * 256 * nw * 8 + (size_t)warps * 32 * 12 + 16; }
+
 template <int NW, int WARPS, bool TOPK = false>
-__global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const FuzzParams P) {
+__global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : NW == 1 ? 6 : NW == 2 ? 9 : 0) fuzz_kernel(const FuzzParams P) {
+    constexpr bool CTA_ROW = NW >= 8;
     extern __shared__ __align__(16) unsigned char dyn[];
     const int lane = lane_id();
     const int w = threadIdx.x >> 5;
-    uint64_t *peq_all = reinterpret_cast<uint64_t *>(dyn) + (size_t)w * 3 * 256 * NW;      // peq[variant][sym * NW + block]
     const int sc_id = P.scorer;
-    const bool need_sorted = sc_id == FZ_TSORT || sc_id == FZ_TRATIO || sc_id == FZ_PTSORT || sc_id == FZ_PTRATIO || sc_id == FZ_WRATIO;
-    const bool need_uniq = sc_id == FZ_TSET || sc_id == FZ_TRATIO || sc_id == FZ_PTSET || sc_id == FZ_PTRATIO || sc_id == FZ_WRATIO;
+    const bool need_sorted = fz_reads_sorted(sc_id), need_uniq = fz_reads_uniq(sc_id);
+    uint64_t *peq_all = nullptr;                                     // one warp: peq[variant][sym * NW + block]
+    uint64_t *peq_v[3];                                    // CTA_ROW: the variants the scorer reads, packed
+    double *sh_s = nullptr; int *sh_j = nullptr, *slot = nullptr;
+    if constexpr (CTA_ROW) {
+        peq_v[0] = reinterpret_cast<uint64_t *>(dyn);
+        peq_v[1] = peq_v[0] + (fz_reads_plain(sc_id) ? 256 * NW : 0);
+        peq_v[2] = peq_v[1] + (need_sorted ? 256 * NW : 0);
+        sh_s = reinterpret_cast<double *>(peq_v[2] + (need_uniq ? 256 * NW : 0));
+        sh_j = reinterpret_cast<int *>(sh_s + WARPS * 32);
+        slot = sh_j + WARPS * 32;
+    } else {
+        peq_all = reinterpret_cast<uint64_t *>(dyn) + (size_t)w * 3 * 256 * NW;
+    }
 
     for (;;) {
-        const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
+        int i;
+        if constexpr (CTA_ROW) i = claim_row_cta(P.counter + blockIdx.y, P.from_ids, P.n_ids, slot);
+        else i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
         if (i < 0) break;
         const GroupRange gr = split_groups(P.n_to, P.n_splits);    // per row: held across rows, it adds spills (2 words)
         int lens[3];
@@ -233,19 +293,26 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
             const int64_t fb = P.F.off[v][i];
             lens[v] = (int)(P.F.off[v][i + 1] - fb);
             if ((v == 1 && !need_sorted) || (v == 2 && !need_uniq)) continue;
-            build_peq<uint64_t, NW>(peq_all + (size_t)v * 256 * NW, P.F.blob[v] + fb, lens[v], P.sym_table);
+            if constexpr (CTA_ROW) {
+                if (v == 0 && !fz_reads_plain(sc_id)) continue;
+                build_peq<uint64_t, NW, true>(peq_v[v], P.F.blob[v] + fb, lens[v], P.sym_table);
+            } else {
+                build_peq<uint64_t, NW>(peq_all + (size_t)v * 256 * NW, P.F.blob[v] + fb, lens[v], P.sym_table);
+            }
         }
         const int la = lens[0], las = lens[1], lau = lens[2];
         const int32_t *atok = P.F.tok_ids + P.F.tok_ptr[i];
         const int na = P.F.tok_ptr[i + 1] - P.F.tok_ptr[i];
         const int na_all = P.F.n_tok_all[i];
         const uint64_t asig = P.F.sig[i];
-        const uint64_t *peq0 = peq_all, *peq1 = peq_all + 256 * NW, *peq2 = peq_all + 2 * 256 * NW;
+        const uint64_t *peq0, *peq1, *peq2;
+        if constexpr (CTA_ROW) { peq0 = peq_v[0]; peq1 = peq_v[1]; peq2 = peq_v[2]; }
+        else { peq0 = peq_all; peq1 = peq_all + 256 * NW; peq2 = peq_all + 2 * 256 * NW; }
 
         WarpArgBest<false> best;
         WarpTopK top;
         if constexpr (TOPK) top.init(P.k); else best.init();
-        for (int g = gr.lo; g < gr.hi; ++g) {
+        for (int g = gr.lo + (CTA_ROW ? w : 0); g < gr.hi; g += CTA_ROW ? WARPS : 1) {
             double cand_s = 0.0; int cand_j = -1;
             do {
                 const int p = g * 32 + lane;
@@ -282,7 +349,7 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
                     double result = 0.0;
                     const double cd = ceil(__dmul_rn((double)(sect_ab_len + sect_ba_len), __dsub_rn(1.0, __ddiv_rn(c, 100.0))));
                     const int dist = ti.n_common == 0 ? (lau + t2.n - 2 * fz_lcs<NW>(peq2, lau, t2))
-                                                      : fz_diff_indel(atok, na, btok, nb, P.tok_blob, P.tok_off);
+                                                      : fz_diff_indel<NW>(peq2, atok, na, btok, nb, P.tok_blob, P.tok_off, P.sym_table);
                     if ((double)dist <= cd) result = fz_norm_distance(dist, sect_ab_len + sect_ba_len, c);
                     if (!sect_len) return result;
                     const double r_ab = fz_norm_distance((sect_len != 0) + ti.ab_len, sect_len + sect_ab_len, c);
@@ -290,7 +357,7 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
                     return fmax(result, fmax(r_ab, r_ba));
                 };
                 auto partial = [&](const uint64_t *peq, int m, const TextRef &t, double c) {
-                    return fz_partial_from_best(fz_partial_best<NW>(peq, m, t), m == 0 && t.n == 0, c);
+                    return fz_partial_from_best(fz_partial_best<NW, CTA_ROW>(peq, m, t), m == 0 && t.n == 0, c);
                 };
                 auto partial_token_ratio = [&](double c) -> double {
                     tok();
@@ -339,6 +406,18 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
             } while (0);
             if constexpr (TOPK) top.offer(cand_s, cand_j);
         }
+        if constexpr (CTA_ROW) {
+            if constexpr (TOPK) {
+                if (merge_cta(top, sh_s, sh_j)) {
+                    const size_t o = ((size_t)blockIdx.y * P.n_from + i) * P.k;
+                    top.store(P.part_idx + o, P.part_score + o);
+                }
+            } else if (merge_cta(best, sh_s, sh_j)) {
+                const size_t o = (size_t)blockIdx.y * P.n_from + i;
+                best.store(P.part_idx + o, P.part_score + o, nullptr);
+            }
+            continue;                                      // (claim_row_cta's barrier ends the row)
+        }
         if constexpr (TOPK) {
             const size_t o = ((size_t)blockIdx.y * P.n_from + i) * P.k;
             top.store(P.part_idx + o, P.part_score + o);
@@ -352,8 +431,13 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) fuzz_kernel(const Fu
 
 template <int NW, bool TOPK>
 static int launch_fuzz(const FuzzParams &P, int sms, cudaStream_t st) {
-    constexpr int WARPS = NW == 1 ? 4 : NW == 2 ? 2 : 1;
-    return launch_rows(fuzz_kernel<NW, WARPS, TOPK>, WARPS, (size_t)WARPS * 3 * 256 * NW * 8, P.n_ids, P.n_splits, sms, st, P);
+    if constexpr (NW >= 8) {
+        constexpr int WARPS = 4;
+        return launch_ctas(fuzz_kernel<NW, WARPS, TOPK>, WARPS, fz_cta_smem(NW, WARPS, P.scorer), P.n_ids, P.n_splits, sms, st, P);
+    } else {
+        constexpr int WARPS = NW == 1 ? 4 : NW == 2 ? 2 : 1;
+        return launch_rows(fuzz_kernel<NW, WARPS, TOPK>, WARPS, (size_t)WARPS * 3 * 256 * NW * 8, P.n_ids, P.n_splits, sms, st, P);
+    }
 }
 
 // the 38 pointers of the C ABI (order: include/pfz.h) -> FuzzParams; part_idx / part_score as the caller's entry point lays them out
@@ -380,7 +464,9 @@ static int run_fuzz(const void *const *ptrs, int32_t n_from, int32_t n_ids, int3
     if (start_rows(P.counter, n_splits, st, &sms)) return 1;
     if (n_words == 1) return launch_fuzz<1, TOPK>(P, sms, st);
     if (n_words == 2) return launch_fuzz<2, TOPK>(P, sms, st);
-    return launch_fuzz<4, TOPK>(P, sms, st);
+    if (n_words == 4) return launch_fuzz<4, TOPK>(P, sms, st);
+    if (n_words == 8) return launch_fuzz<8, TOPK>(P, sms, st);
+    return launch_fuzz<16, TOPK>(P, sms, st);
 }
 
 }  // namespace pfz
@@ -394,7 +480,8 @@ int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, in
                      double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream) {
     PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_argbest: expected 38 pointers, got %d", n_ptrs);
     PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_argbest: unknown scorer %d", scorer);
-    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4, "pfz_fuzz_argbest: n_words %d unsupported (1, 2, 4: strings up to 255 code points)", n_words);
+    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_fuzz_argbest: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
     PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_argbest: n_splits < 1");
     if (n_ids <= 0 || n_to <= 0) return 0;
     return run_fuzz<false>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, n_splits, 1, stream);
@@ -405,7 +492,8 @@ int pfz_fuzz_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32
                   double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k, void *stream) {
     PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_topk: expected 38 pointers, got %d", n_ptrs);
     PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_topk: unknown scorer %d", scorer);
-    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4, "pfz_fuzz_topk: n_words %d unsupported (1, 2, 4: strings up to 255 code points)", n_words);
+    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_fuzz_topk: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
     PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_topk: n_splits < 1");
     PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_fuzz_topk: k=%d unsupported (1..32)", k);
     if (n_ids <= 0 || n_to <= 0) return 0;

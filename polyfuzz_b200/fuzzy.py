@@ -20,7 +20,13 @@ from .strings import pack_strings
 
 SCORER = {"ratio": 0, "QRatio": 1, "partial_ratio": 2, "token_sort_ratio": 3, "token_set_ratio": 4, "token_ratio": 5,
           "partial_token_sort_ratio": 6, "partial_token_set_ratio": 7, "partial_token_ratio": 8, "WRatio": 9}
-MAX_LEN = 255
+MAX_LEN = 1024                                             # code points per from-string (every variant); to-strings: any length
+
+
+def word_class(lens):
+    """64-bit words per from-string mask for the longest of its variants: <= 64 -> 1, <= 128 -> 2, <= 256 -> 4, <= 512 -> 8,
+    else 16 (the 8- and 16-word classes run one CTA per from-row)."""
+    return np.select([lens <= 64, lens <= 128, lens <= 256, lens <= 512], [1, 2, 4, 8], 16).astype(np.int32)
 
 
 def _derive(strings):
@@ -80,11 +86,10 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
     d_tok_blob = _blob_to_dev(tblob); d_tok_off = _to_dev(toff)
     F = _Side(from_list, ftoks, fS, fU, tok_id)
     T = F if same else _Side(to_list, ttoks, tS, tU, tok_id)
-    for side, what in ((F, "from"), (T, "to")):
-        for ln in side.lens:
-            if len(ln) and ln.max() > MAX_LEN:
-                raise ValueError(f"{what}-string {int(ln.argmax())} has {int(ln.max())} code points; the token / partial scorers "
-                                 f"support at most {MAX_LEN}")
+    fl = np.maximum(np.maximum(F.lens[0], F.lens[1]), F.lens[2])
+    if len(fl) and fl.max() > MAX_LEN:
+        raise ValueError(f"from-string {int(fl.argmax())} has {int(fl.max())} code points; the token / partial scorers "
+                         f"support at most {MAX_LEN}")
     # to-side layouts: one length order (by len(b)) for the three variants
     order = np.argsort(T.lens[0], kind="stable").astype(np.int32)
     n_grp = (n_to + 31) // 32
@@ -101,8 +106,7 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
     part_idx = torch.full(shape, -1, dtype=torch.int32, device=dev)
     part_score = torch.zeros(shape, dtype=torch.float64, device=dev)
     counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
-    fl = np.maximum(np.maximum(F.lens[0], F.lens[1]), F.lens[2])
-    classes = np.select([fl <= 64, fl <= 128], [1, 2], 4).astype(np.int32)
+    classes = word_class(fl)
     fblob, foff = F.host[0]
     keep = []
     for lo, hi in _alphabet_batches(fblob, foff):
@@ -113,7 +117,7 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
         for v in range(3):
             _lib.call("pfz_lev_pack", _p(T.dev[v][0]), _p(T.dev[v][1]), _p(d_order), n_to, _p(d_table), _p(packs[v][1]), _p(packs[v][0]),
                       _p(packs[v][2]), _stream())
-        for nw in (1, 2, 4):
+        for nw in (1, 2, 4, 8, 16):
             ids = np.nonzero(classes[lo:hi] == nw)[0].astype(np.int32) + lo
             if len(ids) == 0:
                 continue
