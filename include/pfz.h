@@ -305,6 +305,30 @@ int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t 
 int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
                      int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream);
 
+/* K3b's token tables, built on the device (csrc/pfz_tok.cu).  Replaces the host derivation of s.split(), sorted(), the token
+ * dictionary and the signatures.  Tokens are Python str.split()'s: maximal runs of code points c with not chr(c).isspace().
+ *
+ * pfz_tok_side: one string list (blob int32 code points, offsets int64[n+1], n_chars = offsets[n] code points) ->
+ *   n_all int32[n]                 tokens per string (duplicates counted)
+ *   vocab_blob int32, vocab_off int64[n_occ+1]   the list's distinct tokens in Python string order (code points compared in
+ *                                  turn, a proper prefix first); entries of vocab_off past the vocabulary hold its total length
+ *   tok_ptr int32[n+1], tok_ids int32   each string's distinct token ids (ranks in vocab), ascending
+ *   s_off int64[n+1], s_blob int32  S(s) = all tokens in id order joined by single spaces
+ *   u_off int64[n+1], u_blob int32  U(s) = the distinct tokens joined the same way
+ *   counts_host int64[6] (host memory): n_occ (tokens), vocabulary size, vocabulary code points, S and U code points, tok_ids
+ *   entries.  The blob and tok_ids buffers need max(n_chars, 1) entries, vocab_off n_chars + 1.  Synchronises the stream.
+ * pfz_tok_union: two sorted vocabularies -> their sorted union (u_blob, u_off int64[n_a+n_b+1], entries past the union hold its
+ *   total length; *n_u on the device) and each token's union rank (map_a int32[n_a], map_b int32[n_b]; a monotone map).
+ * pfz_tok_remap: ids_out[j] = map[ids_in[j]] (map NULL: the identity) for the ids of the n strings of tok_ptr, and per string
+ *   the Bloom signature sig = OR over its ids of 1 << (((id * 0x9E3779B1) >> 13) & 63), the product taken in 64 bits.     */
+int pfz_tok_side(const int32_t *blob, const int64_t *offsets, int32_t n, int64_t n_chars, int32_t *n_all, int32_t *vocab_blob,
+                 int64_t *vocab_off, int32_t *tok_ptr, int32_t *tok_ids, int64_t *s_off, int32_t *s_blob, int64_t *u_off,
+                 int32_t *u_blob, int64_t *counts_host, void *stream);
+int pfz_tok_union(const int32_t *a_blob, const int64_t *a_off, int32_t n_a, const int32_t *b_blob, const int64_t *b_off, int32_t n_b,
+                  int32_t *map_a, int32_t *map_b, int32_t *u_blob, int64_t *u_off, int32_t *n_u, void *stream);
+int pfz_tok_remap(const int32_t *tok_ptr, const int32_t *ids_in, int32_t n, const int32_t *map, int32_t *ids_out, uint64_t *sig,
+                  void *stream);
+
 /* top-k sibling of pfz_fuzz_argbest: the k best to-strings per from-string (1 <= k <= 32) under the same candidates and key.
  * Replaces: rapidfuzz process.extract(query, to_list, scorer=..., score_cutoff=..., limit=k), and the sort of the scorer values
  *           of polyfuzz/models/_distance.py:98-99 where the reference takes np.argmax.

@@ -50,6 +50,9 @@ _PROTOS = {
     "pfz_dl_topk": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
                     c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_fuzz_topk":[c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i32, c_i32, c_vp],
+    "pfz_tok_side": [c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    "pfz_tok_union": [c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    "pfz_tok_remap": [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp],
     "pfz_frame_tail_count": [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_frame_tail_copy": [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_rows_to_bf16": [c_vp, c_i32, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp],

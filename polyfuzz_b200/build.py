@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpfz.so")
-SOURCES = ["pfz_core.cu", "pfz_tfidf.cu", "pfz_spcos.cu", "pfz_spcos_block.cu", "pfz_spcos_hash.cu", "pfz_lev.cu", "pfz_fuzz.cu", "pfz_dense.cu", "pfz_assemble.cu"]
+SOURCES = ["pfz_core.cu", "pfz_tfidf.cu", "pfz_spcos.cu", "pfz_spcos_block.cu", "pfz_spcos_hash.cu", "pfz_lev.cu", "pfz_fuzz.cu", "pfz_tok.cu", "pfz_dense.cu", "pfz_assemble.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 

@@ -21,7 +21,8 @@ return the k best under the same key (score desc, index asc), k <= 32.
 
 Two levels: `EditQueries` / `EditTargets` stage a from-list / to-list in HBM once (host packing, length sort,
 alphabet batches); `edit_argbest_staged` only enqueues kernels, so a staged pair can be scored repeatedly
-(bench.py's device-timed leg, the multi-GPU shards) without touching the host lists again.
+(bench.py's device-timed leg, the multi-GPU shards) without touching the host lists again.  `KeptTargets` holds a
+matcher's last staged to-side, which a `re_train=False` call with an equal to-list scores against again.
 """
 import numpy as np
 import torch
@@ -150,6 +151,29 @@ class EditTargets:
         self.slen = torch.empty(self.n, dtype=torch.int32, device=dev)
 
 
+class KeptTargets:
+    """The to-side a matcher staged last (EditTargets for K3, fuzzy.FuzzTargets for K3b), the device it lives on and a copy of
+    the list it was staged from.  Neither depends on the from-list (the alphabet-dependent packing is redone per call), so a
+    later call whose to-list is equal (same length, == element by element) can score against it without staging it again."""
+
+    def __init__(self):
+        self.clear()
+
+    def clear(self):
+        self.key = self.strings = self.staged = None
+
+    def stage(self, kind, to_list, make, reuse):
+        """The kept staging of `to_list` when `reuse` and it matches (kind, device, list); otherwise make(to_list), kept."""
+        key = (kind, torch.cuda.current_device() if torch.cuda.is_available() else -1)
+        if (reuse and self.staged is not None and self.key == key and len(self.strings) == len(to_list)
+                and self.strings == list(to_list)):
+            return self.staged
+        self.clear()
+        staged = make(to_list)
+        self.key, self.strings, self.staged = key, list(to_list), staged
+        return staged
+
+
 def default_splits(n_from, n_grp):
     # ~4 (pattern, to-split) tasks per resident warp: patterns differ in length, finer tasks balance the tail
     want = 4 * 132 * 48
@@ -226,11 +250,12 @@ def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=Fal
 
 
 def edit_argbest(from_list, to_list, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0,
-                 want_matrix=False, n_splits=None, dl_gate=True):
-    """Host lists in, device tensors out (see edit_argbest_staged)."""
+                 want_matrix=False, n_splits=None, dl_gate=True, kept=None, reuse=False):
+    """Host lists in, device tensors out (see edit_argbest_staged).  kept (KeptTargets): where the staged to-side is kept;
+    reuse: take it from there when it was staged from an equal to_list."""
     _dev()
     Q = EditQueries(from_list)
-    T = EditTargets(to_list)
+    T = kept.stage(("k3", 0), to_list, EditTargets, reuse) if kept is not None else EditTargets(to_list)
     return edit_argbest_staged(Q, T, metric, score_cutoff, exclude_self, self_shift, want_matrix, n_splits, dl_gate=dl_gate)
 
 
@@ -282,12 +307,13 @@ def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=Fal
     return idx, score
 
 
-def edit_topk(from_list, to_list, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, dl_gate=True):
-    """Host lists in, device tensors out (see edit_topk_staged)."""
+def edit_topk(from_list, to_list, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, dl_gate=True,
+              kept=None, reuse=False):
+    """Host lists in, device tensors out (see edit_topk_staged); kept and reuse as in edit_argbest."""
     k = check_top_n(k)
     _dev()
     Q = EditQueries(from_list)
-    T = EditTargets(to_list)
+    T = kept.stage(("k3", 0), to_list, EditTargets, reuse) if kept is not None else EditTargets(to_list)
     return edit_topk_staged(Q, T, k, metric, score_cutoff, exclude_self, self_shift, n_splits, dl_gate=dl_gate)
 
 

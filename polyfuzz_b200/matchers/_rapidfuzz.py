@@ -81,29 +81,39 @@ def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
                               + "); polyfuzz_b200 has no CPU fallback")
 
 
-def _argbest(from_list, targets, metric, cutoff, self_match, distributed):
+def _argbest(from_list, targets, metric, cutoff, self_match, distributed, kept=None, reuse=False):
     """Best to-string per from-string on this GPU, or -- distributed=True under torchrun -- on the to_list row-block of every
     rank followed by ONE all-gather of the per-shard bests and the canonical merge (score desc, global index asc): all ranks
-    get the single-GPU result (SURVEY.md 8e; the reference's own fan-out is per from-row, polyfuzz/models/_rapidfuzz.py:92-95)."""
+    get the single-GPU result (SURVEY.md 8e; the reference's own fan-out is per from-row, polyfuzz/models/_rapidfuzz.py:92-95).
+    kept / reuse: the matcher's kept to-side (editdist.KeptTargets; each rank keeps its own shard) and whether it may serve
+    this call."""
     comm = get_comm() if distributed else None
     token_scorer = metric in fuzzy.SCORER and metric != "ratio"
     if comm is None:
         if token_scorer:
-            return fuzzy.fuzz_argbest(from_list, targets, metric, cutoff, exclude_self=self_match) + (None,)
-        return editdist.edit_argbest(from_list, targets, metric, cutoff, exclude_self=self_match)
+            return fuzzy.fuzz_argbest(from_list, targets, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse) + (None,)
+        return editdist.edit_argbest(from_list, targets, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
     lo, hi = shard_bounds(len(targets), comm.world_size, comm.rank)
     if token_scorer:
-        bi, bs = fuzzy.fuzz_argbest(from_list, targets[lo:hi], metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
+        bi, bs = fuzzy.fuzz_argbest(from_list, targets[lo:hi], metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo,
+                                    kept=kept, reuse=reuse)
         bd = torch_full_like_int(bi)
     else:
         Q = editdist.EditQueries(from_list)
-        T = editdist.EditTargets(targets[lo:hi])
+        T = _shard_targets(targets[lo:hi], lo, kept, reuse)
         bi, bs, bd = editdist.edit_argbest_staged(Q, T, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
     gi, gs, gd = comm.all_gather_best(bi, bs, bd)
     return editdist.lev_merge(gi, gs, gd)
 
 
-def _topk(from_list, targets, metric, cutoff, self_match, distributed, k):
+def _shard_targets(shard, lo, kept, reuse):
+    """This rank's staged K3 to-shard: the kept one when it may serve, else a new EditTargets (kept when a holder is given)."""
+    if kept is None:
+        return editdist.EditTargets(shard)
+    return kept.stage(("k3", lo), shard, lambda lst: editdist.EditTargets(lst), reuse)
+
+
+def _topk(from_list, targets, metric, cutoff, self_match, distributed, k, kept=None, reuse=False):
     """Top-k sibling of _argbest: the k best to-strings per from-string (device idx int32[n, k], -1 = empty slot, and score
     float64[n, k]) on this GPU, or -- distributed=True under torchrun -- per to_list row-block followed by ONE all-gather of the
     per-shard lists and the canonical merge, as TF-IDF and Embeddings do: all ranks get the single-GPU result."""
@@ -111,14 +121,15 @@ def _topk(from_list, targets, metric, cutoff, self_match, distributed, k):
     token_scorer = metric in fuzzy.SCORER and metric != "ratio"
     if comm is None:
         if token_scorer:
-            return fuzzy.fuzz_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match)
-        return editdist.edit_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match)
+            return fuzzy.fuzz_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
+        return editdist.edit_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
     lo, hi = shard_bounds(len(targets), comm.world_size, comm.rank)
     if token_scorer:
-        idx, val = fuzzy.fuzz_topk(from_list, targets[lo:hi], k, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
+        idx, val = fuzzy.fuzz_topk(from_list, targets[lo:hi], k, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo,
+                                   kept=kept, reuse=reuse)
     else:
         Q = editdist.EditQueries(from_list)
-        T = editdist.EditTargets(targets[lo:hi])
+        T = _shard_targets(targets[lo:hi], lo, kept, reuse)
         idx, val = editdist.edit_topk_staged(Q, T, k, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
     gi, gv = comm.all_gather_topk(idx.contiguous(), val.contiguous())
     return merge_topk_any(gi, gv, k)
@@ -139,7 +150,28 @@ def torch_full_like_int(t):
     import torch
     return torch.full_like(t, -1)
 
-class RapidFuzz(BaseMatcher):
+
+class _KeepsTargets:
+    """A matcher that keeps the to-side it staged last (editdist.KeptTargets): a call with re_train=False whose to-list equals
+    the kept one (same length, == element by element) scores against it without staging it again -- PolyFuzz.transform's
+    `match(new, self.to_list, re_train=False)`.  A self-match's list counts as its to-list.  Pickling drops the device state;
+    the first call after loading stages again."""
+
+    def _kept(self):
+        kept = self.__dict__.get("_kept_targets")
+        if kept is None:
+            kept = self._kept_targets = editdist.KeptTargets()
+        return kept
+
+    def __getstate__(self):
+        st = dict(self.__dict__)
+        st.pop("_kept_targets", None)
+        return st
+
+    def __setstate__(self, st):
+        self.__dict__.update(st)
+
+class RapidFuzz(_KeepsTargets, BaseMatcher):
     """Edit-distance matcher (GPU).  Arguments as in the reference: n_jobs (accepted, ignored -- the GPU
     scores all pairs in one launch), score_cutoff in [0,1], scorer (default fuzz.WRatio, as the reference), model_id.
     top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given."""
@@ -156,9 +188,11 @@ class RapidFuzz(BaseMatcher):
         self.equal_lists = False
         self.n_jobs = n_jobs
 
-    def match(self, from_list: List[str], to_list: List[str] = None, **kwargs) -> pd.DataFrame:
+    def match(self, from_list: List[str], to_list: List[str] = None, re_train: bool = True, **kwargs) -> pd.DataFrame:
         """(from, best to, score/100); no candidate with score >= score_cutoff -> (from, None, 0.0)
-        (polyfuzz/models/_rapidfuzz.py:106-113).  top_n > 1: the k best, an empty slot is (None, 0.0)."""
+        (polyfuzz/models/_rapidfuzz.py:106-113).  top_n > 1: the k best, an empty slot is (None, 0.0).
+        re_train=False: score against the kept to-side when to_list equals the list it was staged from (the frame is the
+        same as a fresh call's); any call that stages keeps its to-side."""
         self_match = to_list is None
         targets = from_list if self_match else to_list
         unit = self._metric in ("norm_lev", "norm_osa", "norm_dl")             # scores already on 0..1
@@ -166,9 +200,9 @@ class RapidFuzz(BaseMatcher):
         cutoff = self.score_cutoff / 100.0 if unit else self.score_cutoff
         top_n = clip_top_n(self.top_n, to_list)
         if top_n > 1:
-            idx, score = _topk(from_list, targets, self._metric, cutoff, self_match, self.distributed, top_n)
+            idx, score = _topk(from_list, targets, self._metric, cutoff, self_match, self.distributed, top_n, self._kept(), not re_train)
             return _topk_frame(from_list, targets, idx.cpu().numpy(), score.cpu().numpy() / scale)
-        idx, score, _ = _argbest(from_list, targets, self._metric, cutoff, self_match, self.distributed)
+        idx, score, _ = _argbest(from_list, targets, self._metric, cutoff, self_match, self.distributed, self._kept(), not re_train)
         idx = idx.cpu().numpy(); score = score.cpu().numpy() / scale
         to_arr = np.empty(len(targets) + 1, dtype=object); to_arr[:-1] = targets; to_arr[-1] = None
         sel = np.where(idx >= 0, idx, len(targets))
@@ -176,7 +210,7 @@ class RapidFuzz(BaseMatcher):
                              "Similarity": np.where(idx >= 0, score, 0.0)})
 
 
-class EditDistance(BaseMatcher):
+class EditDistance(_KeepsTargets, BaseMatcher):
     """Edit-distance matcher with the reference's EditDistance surface (n_jobs, scorer, model_id, normalize):
     Similarity is the scorer's raw value (fuzz.ratio: 0..100, Levenshtein / OSA / DL / Jaro / Jaro-Winkler: 0..1) of the best to-string,
     min-max normalised over the column when `normalize` (polyfuzz/models/_distance.py:83-86).
@@ -197,7 +231,8 @@ class EditDistance(BaseMatcher):
         self.equal_lists = False
         self.n_jobs = n_jobs
 
-    def match(self, from_list: List[str], to_list: List[str] = None, **kwargs) -> pd.DataFrame:
+    def match(self, from_list: List[str], to_list: List[str] = None, re_train: bool = True, **kwargs) -> pd.DataFrame:
+        """re_train as in RapidFuzz.match."""
         self_match = to_list is None
         targets = from_list if self_match else to_list
         if len(targets) - (1 if self_match else 0) < 1:
@@ -207,7 +242,7 @@ class EditDistance(BaseMatcher):
         no_cut = 0.0 if self._metric in fuzzy.SCORER and self._metric != "ratio" else float("-inf")
         top_n = clip_top_n(self.top_n, to_list)
         if top_n > 1:
-            idx, score = _topk(from_list, targets, self._metric, no_cut, self_match, self.distributed, top_n)
+            idx, score = _topk(from_list, targets, self._metric, no_cut, self_match, self.distributed, top_n, self._kept(), not re_train)
             idx = idx.cpu().numpy(); score = score.cpu().numpy()
             if self.normalize:
                 filled = idx >= 0
@@ -215,7 +250,7 @@ class EditDistance(BaseMatcher):
                 with np.errstate(invalid="ignore", divide="ignore"):
                     score = np.where(filled, (score - lo) / (hi - lo), 0.0)
             return _topk_frame(from_list, targets, idx, score)
-        idx, score, _ = _argbest(from_list, targets, self._metric, no_cut, self_match, self.distributed)
+        idx, score, _ = _argbest(from_list, targets, self._metric, no_cut, self_match, self.distributed, self._kept(), not re_train)
         idx = idx.cpu().numpy(); score = score.cpu().numpy()
         to_arr = np.empty(len(targets), dtype=object); to_arr[:] = targets
         matches = pd.DataFrame({"From": pd.Series(list(from_list), dtype=object), "To": pd.Series(to_arr[idx], dtype=object),
