@@ -233,7 +233,9 @@ int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32
 
 /* scores the from-strings listed in from_ids (all of one word class: n_words = 0 -> length <= 32 (one
  * 32-bit word), 1/2/4/8/16 -> length <= 64*n_words) against every to-string.
- *   metric: PFZ_METRIC_*; for NORM_LEV / RATIO / JARO / JARO_WINKLER / NORM_OSA a candidate needs score >= score_cutoff
+ *   metric: PFZ_METRIC_*; for NORM_LEV / JARO / JARO_WINKLER / NORM_OSA a candidate needs score >= score_cutoff; for RATIO
+ *           rapidfuzz's two steps: ns = 1 - indel/(|a|+|b|) >= score_cutoff/100 (fuzz.ratio) and score = ns*100 >= score_cutoff
+ *           (extractOne), which differ whenever (ns*100)/100 != ns -- e.g. ns = 17/25 is rejected at score_cutoff 68.0
  *   exclude_self: skip to-row == from-row + self_shift
  *   part_*: [n_splits][n_from] partial bests (merge with pfz_lev_merge); ties -> lowest to-index;
  *           part_dist holds the distance, or for JARO / JARO_WINKLER the number of matching characters
@@ -254,8 +256,8 @@ int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int3
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits,
                   int32_t n_from, int32_t *best_idx, double *best_score, int32_t *best_dist, void *stream);
 
-/* top-k sibling of pfz_lev_argbest: the k best to-strings per from-string (1 <= k <= 32), same candidates (score >= score_cutoff,
- * to-row == from-row + self_shift excluded when exclude_self) and key (score desc, to-index asc).
+/* top-k sibling of pfz_lev_argbest: the k best to-strings per from-string (1 <= k <= 32), same candidates (the cutoff tests
+ * above, to-row == from-row + self_shift excluded when exclude_self) and key (score desc, to-index asc).
  * Replaces: rapidfuzz process.extract(query, to_list, scorer, limit=k), and the sort of the scorer values of
  *           polyfuzz/models/_distance.py:98-99 where the reference takes np.argmax.
  *   metric: NORM_LEV, RATIO, JARO, JARO_WINKLER or NORM_OSA; there is no distance output and no matrix.
@@ -301,7 +303,12 @@ int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t 
  *       length), sym_table uint8[0x110000], for each variant {packed, grp_word_off, slen}
  *       (pfz_lev_pack layouts of b, S(b), U(b) in ONE length order), sorig int32[n_to], tok_blob uint32, tok_off int64[n_tok+1],
  *       part_idx int32[n_splits][n_from], part_score float64[n_splits][n_from], counter int32[n_splits], reserved (NULL).
- * Best = first to-string (lowest index) with the maximal score >= score_cutoff; merge the splits with pfz_lev_merge.          */
+ * Best = first to-string (lowest index) with the maximal score >= score_cutoff; merge the splits with pfz_lev_merge.
+ * The cutoff reaches the scorer as in rapidfuzz: ratio (also inside token_sort_ratio, token_ratio, QRatio, WRatio) keeps
+ * ns = 1 - indel/(|a|+|b|) only if ns >= score_cutoff/100, and partial_ratio (also inside the partial_token_* scorers and
+ * WRatio) keeps its best window's ns only if ns >= score_cutoff/100 and ns*100 >= score_cutoff; the token-set parts test
+ * 100 - 100*dist/lensum >= score_cutoff once.  So a pair is rejected at a cutoff equal to its own score whenever
+ * (ns*100)/100 > ns in doubles, and WRatio's internal cutoffs (max(c, end_ratio)/0.9, /0.95) apply the same rule.          */
 int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
                      int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream);
 

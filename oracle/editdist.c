@@ -126,7 +126,18 @@ int oracle_editdist_matrix(const uint32_t *fb, const int64_t *fo, int32_t n_from
     return 0;
 }
 
-/* per from-row best match: first index with maximal score among score >= cutoff
+/* RATIO's cutoff has rapidfuzz's two steps: fuzz.ratio keeps ns = 1 - d/m only if ns >= cutoff/100 and returns ns*100,
+ * then extractOne keeps that score only if it is >= cutoff.  The two disagree whenever (ns*100)/100 != ns in doubles.
+ * NORM_LEV (Levenshtein.normalized_similarity) has no /100 step: one test. */
+static int passes_cutoff(int metric, int32_t d, int32_t la, int32_t lb, double s, double score_cutoff) {
+    if (metric == ORACLE_NORM_LEV) return s >= score_cutoff;
+    if (metric != ORACLE_RATIO) return 1;
+    int32_t m = la + lb;
+    double ns = m ? 1.0 - (double)d / (double)m : 1.0;
+    return ns >= score_cutoff / 100.0 && s >= score_cutoff;
+}
+
+/* per from-row best match: first index with maximal score among the candidates that pass the cutoff
  * (metric LEV/INDEL: score = -distance, cutoff ignored).  exclude_self: skip j == i + self_shift. */
 int oracle_editdist_argbest(const uint32_t *fb, const int64_t *fo, int32_t n_from,
                             const uint32_t *tb, const int64_t *to, int32_t n_to,
@@ -151,7 +162,7 @@ int oracle_editdist_argbest(const uint32_t *fb, const int64_t *fo, int32_t n_fro
                 const uint32_t *b = tb + to[j]; int32_t lb = (int32_t)(to[j + 1] - to[j]);
                 int32_t d = dist_of(metric, a, la, b, lb, row);
                 double s = score_of(metric, d, la, lb);
-                if ((metric == ORACLE_NORM_LEV || metric == ORACLE_RATIO) && !(s >= score_cutoff)) continue;
+                if (!passes_cutoff(metric, d, la, lb, s, score_cutoff)) continue;
                 if (bi < 0 || s > bs) { bi = j; bs = s; bd = d; }
             }
             best_idx[i] = bi; best_score[i] = bi < 0 ? 0.0 : bs; best_dist[i] = bd;

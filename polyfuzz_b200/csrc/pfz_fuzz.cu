@@ -66,10 +66,12 @@ __device__ __forceinline__ double fz_norm_distance(int dist, int lensum, double 
     const double sc = lensum ? __dsub_rn(100.0, __ddiv_rn(__dmul_rn(100.0, (double)dist), (double)lensum)) : 100.0;
     return sc >= cutoff ? sc : 0.0;
 }
+// partial_ratio's two cutoff steps: its windows are scored at cutoff / 100 (best_ns is kept only if best_ns >= cutoff / 100),
+// then the result best_ns * 100 only if it is >= cutoff -- as fz_ratio, they disagree whenever (ns * 100) / 100 != ns
 __device__ __forceinline__ double fz_partial_from_best(double best_ns, bool both_empty, double cutoff) {
     if (both_empty) return 100.0;
     const double res = __dmul_rn(best_ns, 100.0);
-    return res >= cutoff ? res : 0.0;
+    return best_ns >= __ddiv_rn(cutoff, 100.0) && res >= cutoff ? res : 0.0;
 }
 
 // ---- bit-parallel LCS over NW 64-bit blocks ------------------------------------------------------------------------------------

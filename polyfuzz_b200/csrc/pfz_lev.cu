@@ -20,6 +20,7 @@
 // loop), dispatch_words (n_words -> <W, NW>) and run_k3 (the body of the C entry points).
 #include "pfz_common.cuh"
 #include <math_constants.h>
+#include <cmath>
 
 namespace pfz {
 
@@ -63,6 +64,7 @@ struct LevParams {
     const uint8_t *sym_table;
     const uint32_t *packed; const int64_t *grp_word_off; const int32_t *slen; const int32_t *sorig; int n_to;
     int metric; double cutoff; int exclude_self; int64_t self_shift;
+    double ratio_min_ns;                // RATIO: its cutoff as one test ns >= ratio_min_ns (ratio_min_ns_of)
     int n_splits;                       // to-groups are split over blockIdx.y
     int32_t *part_idx; double *part_score; int32_t *part_dist;     // [n_splits][n_from]
     int32_t *matrix; int64_t matrix_ld;                           // optional full matrix [n_from][n_to]
@@ -70,10 +72,27 @@ struct LevParams {
     int k;                              // top-k epilogue: list length; part_idx / part_score are [n_splits][n_from][k]
 };
 
+__device__ __forceinline__ double ratio_ns(int d, int la, int lb) {      // Indel.normalized_similarity
+    const int m = la + lb;
+    return m ? 1.0 - (double)d / (double)m : 1.0;
+}
+
 __device__ __forceinline__ double score_of(int metric, int d, int la, int lb) {
     if (metric == PFZ_METRIC_NORM_LEV) { const int m = max(la, lb); return m ? 1.0 - (double)d / (double)m : 1.0; }
-    if (metric == PFZ_METRIC_RATIO) { const int m = la + lb; return m ? (1.0 - (double)d / (double)m) * 100.0 : 100.0; }
     return -(double)d;                  // raw distances: best = smallest
+}
+
+// RATIO's cutoff c in rapidfuzz's two steps: fuzz.ratio keeps ns only if ns >= c / 100 and returns ns * 100, then extractOne
+// keeps that score only if ns * 100 >= c.  The steps disagree whenever (ns * 100) / 100 != ns (ns = 17/25 is rejected at
+// c = 68.0).  Rounding is monotone, so {ns : ns * 100 >= c} is {ns >= t} for the least double t in it, and the two steps are
+// the one test ns >= max(c / 100, t), found here once per launch.
+static double ratio_min_ns_of(double c) {
+    const double q = c / 100.0;
+    if (!std::isfinite(q)) return q;                       // -inf: every pair, +inf / NaN: none (as both steps)
+    double t = q;
+    while (!(t * 100.0 >= c)) t = std::nextafter(t, HUGE_VAL);
+    while (std::nextafter(t, -HUGE_VAL) * 100.0 >= c) t = std::nextafter(t, -HUGE_VAL);
+    return t > q ? t : q;
 }
 
 // the row's slot of part_*: its k best (TOPK) or its arg-best
@@ -244,12 +263,19 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
             }
             if (have) {
                 if (P.matrix) P.matrix[(int64_t)i * P.matrix_ld + orig] = dist;
-                // OSA scores like Levenshtein: NORM_OSA takes NORM_LEV's expression and cutoff, raw OSA is a distance
-                const double sc = OSA ? score_of(P.metric == PFZ_METRIC_NORM_OSA ? PFZ_METRIC_NORM_LEV : PFZ_METRIC_LEV, dist, m, n)
-                                      : score_of(P.metric, dist, m, n);
                 bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift);
-                if ((OSA ? P.metric == PFZ_METRIC_NORM_OSA : (P.metric == PFZ_METRIC_NORM_LEV || P.metric == PFZ_METRIC_RATIO)) &&
-                    !(sc >= P.cutoff)) ok = false;
+                double sc;
+                if constexpr (LCS) {                    // RATIO: ns * 100 with the two-step cutoff; INDEL: the distance
+                    const bool ratio = P.metric == PFZ_METRIC_RATIO;
+                    const double ns = ratio ? ratio_ns(dist, m, n) : 0.0;
+                    sc = ratio ? ns * 100.0 : -(double)dist;
+                    if (ratio && !(ns >= P.ratio_min_ns)) ok = false;
+                } else {
+                    // OSA scores like Levenshtein: NORM_OSA takes NORM_LEV's expression and cutoff, raw OSA is a distance
+                    sc = OSA ? score_of(P.metric == PFZ_METRIC_NORM_OSA ? PFZ_METRIC_NORM_LEV : PFZ_METRIC_LEV, dist, m, n)
+                             : score_of(P.metric, dist, m, n);
+                    if ((OSA ? P.metric == PFZ_METRIC_NORM_OSA : P.metric == PFZ_METRIC_NORM_LEV) && !(sc >= P.cutoff)) ok = false;
+                }
                 if constexpr (TOPK) { cand_s = sc; cand_j = ok ? orig : -1; }
                 else if (ok) best.offer(sc, orig, dist);
             }
@@ -634,7 +660,8 @@ static int run_k3(const char *fn, const uint32_t *from_blob, const int64_t *from
     int sms = 0;
     if (start_rows(counter, n_splits, st, &sms)) return 1;
     LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
-                exclude_self, self_shift, n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from, counter, k};
+                exclude_self, self_shift, ratio_min_ns_of(score_cutoff), n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from,
+                counter, k};
     return launch_class<TOPK>(P, gate, n_words, sms, st);
 }
 
