@@ -322,7 +322,10 @@ __global__ void __launch_bounds__(DENSE_THREADS, 1) dense_cos_topk_kernel(const 
     if (MCAST) cluster_sync_all();                                       // no CTA exits while its peer may still write into it
 }
 
-// rows -> l2-normalised bf16 (fp64 or fp32 in); zero rows stay zero.  One warp per row.
+// rows -> bf16 (fp64 or fp32 in), zero padded to d_pad.  normalize = 0: bf16(float(x)), rounded to nearest even.
+// normalize = 1: a faithful bf16 rounding of x / ||x|| for every element of magnitude >= 2^-100, and the same bits for
+// x and 2^e x: the row is first scaled by 2^-E, E = ilogb(max |x|), which is exact, so the fp32 sum of squares lies in
+// [1, 4 d] and neither overflows nor leaves the normal range at any input scale.  Zero rows stay zero.  One warp per row.
 template <typename T>
 __global__ void __launch_bounds__(256) rows_normalize_bf16_kernel(const T *__restrict__ x, int64_t ld, int n_rows, int d, int d_pad, int normalize,
                                                                   __nv_bfloat16 *__restrict__ out) {
@@ -330,14 +333,22 @@ __global__ void __launch_bounds__(256) rows_normalize_bf16_kernel(const T *__res
     const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
     for (int r = gw; r < n_rows; r += nw) {
         const T *row = x + (int64_t)r * ld;
-        float ss = 0.f;
-        if (normalize) {
-            for (int c = lane; c < d; c += 32) { const float v = (float)row[c]; ss += v * v; }
-#pragma unroll
-            for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(FULL, ss, o);
+        __nv_bfloat16 *o = out + (int64_t)r * d_pad;
+        if (!normalize) {
+            for (int c = lane; c < d_pad; c += 32) o[c] = __float2bfloat16(c < d ? (float)row[c] : 0.f);
+            continue;
         }
-        const float inv = (normalize && ss > 0.f) ? rsqrtf(ss) : 1.f;
-        for (int c = lane; c < d_pad; c += 32) out[(int64_t)r * d_pad + c] = __float2bfloat16(c < d ? (float)row[c] * inv : 0.f);
+        double mx = 0.0;
+        for (int c = lane; c < d; c += 32) mx = fmax(mx, fabs((double)row[c]));
+#pragma unroll
+        for (int s = 16; s; s >>= 1) mx = fmax(mx, __shfl_xor_sync(FULL, mx, s));
+        const int e = mx > 0.0 ? -ilogb(mx) : 0;
+        float ss = 0.f;
+        for (int c = lane; c < d; c += 32) { const float v = (float)ldexp((double)row[c], e); ss += v * v; }
+#pragma unroll
+        for (int s = 16; s; s >>= 1) ss += __shfl_xor_sync(FULL, ss, s);
+        const float inv = ss > 0.f ? rsqrtf(ss) : 1.f;
+        for (int c = lane; c < d_pad; c += 32) o[c] = __float2bfloat16(c < d ? (float)ldexp((double)row[c], e) * inv : 0.f);
     }
 }
 

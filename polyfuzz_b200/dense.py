@@ -1,6 +1,7 @@
 """K4 host driver: dense cosine top-k of pre-computed embeddings on the tensor cores (include/pfz.h,
-pfz_rows_to_bf16 + pfz_dense_cos_topk).  Inputs are rounded to bf16 (after l2 normalisation in fp32);
-products accumulate in fp32 (wgmma register accumulators); the ranking key is (score desc, index asc) on those fp32 values.
+pfz_rows_to_bf16 + pfz_dense_cos_topk).  Inputs are l2-normalised and rounded to bf16 (to_bf16_rows); products
+accumulate in fp32 (wgmma register accumulators); the ranking key is (score desc, index asc) on those fp32 values, and a
+to-row is eligible iff its score > float32(min_similarity) (and it is not the diagonal of a self-match).
 The exact mode (stage_exact + dense_topk_exact) returns the canonical fp64 top-k instead: an fp16 tensor-core filter pass,
 fp64 re-scoring of its candidates with a per-row certificate, and a brute-force fp64 pass for the rows not certified."""
 import numpy as np
@@ -13,7 +14,10 @@ SM_COUNT = 132                     # H100 SXM
 
 
 def to_bf16_rows(x, normalize=True):
-    """ndarray / tensor [n, d] (float32/float64) -> device bf16 [n, d_pad] (d_pad = d rounded up to 8)."""
+    """ndarray / tensor [n, d] (float32/float64) -> (device bf16 [n, d_pad], the device input), d_pad = d rounded up to 8
+    (at least 8), padding columns +0.  normalize=False: each element is float32(x) rounded to the nearest even bf16.
+    normalize=True: each element is a faithful bf16 rounding of x / ||x|| (one of its two bf16 neighbours) wherever that is
+    at least 2^-100 in magnitude, and x and 2^e x stage to the same bits at any finite scale; zero rows stay zero."""
     dev = _dev()
     if isinstance(x, np.ndarray):
         if x.dtype not in (np.float32, np.float64):
