@@ -446,14 +446,16 @@ int pfz_dense_topn_select(const int32_t *cand_idx, const double *cand_val, const
  *           and the `Similarity < 0.001 -> 0, To -> None` rule of :119-123).  ASCII string lists only (bytes == code points).
  * Column-major entries e = r*n + i (r = rank 0..k-1, i = from-row):
  *   sims    float64[k*n]     np.round(score, 3), 0 where the slot is empty or rounds below 0.001
- *   lens_pos int32[k*n + 1]  on return the EXCLUSIVE prefix of the matched strings' byte lengths (last entry = total bytes)
+ *   lens_pos int64[k*n + 1]  on return the EXCLUSIVE prefix of the matched strings' byte lengths (last entry = total bytes).
+ *                            64-bit: a frame's matched strings may total 2 GiB or more (e.g. 1M rows x top 25 x 90 bytes)
  *   bitmap  uint32[k * ceil(n/32)]   Arrow validity bits (bit i of column r)
- *   ws: >= pfz_scan_ws_bytes(k*n + 1) bytes.
+ *   ws: ws_bytes >= pfz_frame_tail_ws_bytes(k*n) bytes (the scan's temporary storage; -1 on error).
  * then, with the total known to the caller: offsets int64[k*(n+1)] (relative to each column's start: Arrow large_string, what
- * pandas' Arrow-backed str dtype holds) and the UTF-8 bytes.   */
+ * pandas' Arrow-backed str dtype holds) and the UTF-8 bytes, both addressed with the 64-bit positions.   */
+int64_t pfz_frame_tail_ws_bytes(int64_t n_entries);
 int pfz_frame_tail_count(const int32_t *top_idx, const double *top_val, int32_t n, int32_t k, const int64_t *to_offsets, double *sims,
-                         int32_t *lens_pos, uint32_t *bitmap, void *ws, void *stream);
-int pfz_frame_tail_copy(const int32_t *top_idx, int32_t n, int32_t k, const int32_t *to_blob, const int64_t *to_offsets, const int32_t *pos,
+                         int64_t *lens_pos, uint32_t *bitmap, void *ws, int64_t ws_bytes, void *stream);
+int pfz_frame_tail_copy(const int32_t *top_idx, int32_t n, int32_t k, const int32_t *to_blob, const int64_t *to_offsets, const int64_t *pos,
                         int64_t *offsets, uint8_t *data, void *stream);
 
 #ifdef __cplusplus

@@ -15,7 +15,9 @@ def assemble(from_list, to_list, top_idx, top_val):
     for r in range(k):
         sims = np.round(np.asarray(top_val[:, r], dtype=np.float64), 3)
         names = [to_list[j] if j >= 0 else None for j in top_idx[:, r]]
-        low = sims < 0.001
+        # an empty slot of the top-k arrays (index -1) is blank whatever score it carries; the reference has no empty
+        # slots, and the kernels write them as (-1, 0.0)
+        low = (sims < 0.001) | (np.asarray(top_idx[:, r]) < 0)
         sims = np.where(low, 0.0, sims)
         names = [None if l else nm for l, nm in zip(low, names)]
         cols["To" if r == 0 else f"To_{r + 1}"] = names

@@ -53,7 +53,8 @@ _PROTOS = {
     "pfz_tok_side": [c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_tok_union": [c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_tok_remap": [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp],
-    "pfz_frame_tail_count": [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    "pfz_frame_tail_ws_bytes": [c_i64],
+    "pfz_frame_tail_count": [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp],
     "pfz_frame_tail_copy": [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_rows_to_bf16": [c_vp, c_i32, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp],
     "pfz_dense_cos_topk": [c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp],
@@ -71,7 +72,7 @@ _PROTOS = {
 }
 _RESTYPES = {"pfz_last_error": ctypes.c_char_p, "pfz_scan_ws_bytes": c_i64, "pfz_launch_count": c_i64, "pfz_spcos_block_ws_bytes": c_i64,
              "pfz_spcos_block_gcnt_offset": c_i64,
-             "pfz_dense_exact_fallback_ws_bytes": c_i64}
+             "pfz_dense_exact_fallback_ws_bytes": c_i64, "pfz_frame_tail_ws_bytes": c_i64}
 
 
 def exported_names():

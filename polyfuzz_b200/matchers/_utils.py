@@ -141,10 +141,14 @@ def assemble_matches_device(from_arrow, to_blob, to_off, top_idx, top_val) -> pd
     nw = (n + 31) // 32
     top_idx = top_idx.contiguous(); top_val = top_val.contiguous()
     sims = torch.empty(k * n, dtype=torch.float64, device=dev)
-    pos = torch.empty(k * n + 1, dtype=torch.int32, device=dev)
+    pos = torch.empty(k * n + 1, dtype=torch.int64, device=dev)                 # byte positions: a frame may hold >= 2 GiB of strings
     bitmap = torch.empty(k * nw, dtype=torch.int32, device=dev)
-    ws = _ws(_lib.load().pfz_scan_ws_bytes(k * n + 1))
-    _lib.call("pfz_frame_tail_count", _p(top_idx), _p(top_val), n, k, _p(to_off), _p(sims), _p(pos), _p(bitmap), _p(ws), _stream())
+    ws_bytes = _lib.load().pfz_frame_tail_ws_bytes(k * n)
+    if ws_bytes < 0:
+        raise RuntimeError("pfz_frame_tail_ws_bytes failed")
+    ws = _ws(ws_bytes)
+    _lib.call("pfz_frame_tail_count", _p(top_idx), _p(top_val), n, k, _p(to_off), _p(sims), _p(pos), _p(bitmap), _p(ws), ws.numel(),
+              _stream())
     total = int(pos[-1].item())                               # the one host sync of the tail (everything before it is done by then)
     offsets = torch.empty(k * (n + 1), dtype=torch.int64, device=dev)           # large_string offsets: pandas wraps them without a cast
     data = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)

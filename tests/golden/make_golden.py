@@ -12,7 +12,14 @@ What is recorded (SURVEY.md section 8c "Golden vectors"):
                       cosine_similarity(method="sklearn") top-10 indices + 3-dp scores
   clean_survivors.json  exhaustive probe of _clean_string over all code points
   dense_c1.npz        reference tests/from_list.npy|to_list.npy + reference sklearn-branch result
+  k1_edges.npz        reference TFIDF._extract_tf_idf on the lists of tests/k1_cases.py, at the places where the GPU
+                      vectoriser changes path: rows of 255..257 and 8 191..8 192 n-gram slots, a code space of exactly
+                      2^24 and one just above it, n-gram codes >= 2^63; fit CSR of both lists, idf, vocabulary, the CSR
+                      of a transformed list with unseen symbols and n-grams, and a digest of the inputs.
+                      Write only this fixture:  python tests/golden/make_golden.py --k1-edges
 """
+import io
+import zipfile
 import json
 import os
 import sys
@@ -46,6 +53,35 @@ def csr_parts(prefix, m, out):
 
 def df_to_json(df):
     return {c: [None if (isinstance(v, float) and np.isnan(v)) else v for v in df[c].tolist()] for c in df.columns}
+
+
+def savez_fixed(path, arrays):
+    """np.savez_compressed with fixed zip timestamps, so that regenerating a fixture is byte-identical."""
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_DEFLATED) as z:
+        for name, arr in arrays.items():
+            buf = io.BytesIO()
+            np.lib.format.write_array(buf, np.asarray(arr), allow_pickle=False)
+            info = zipfile.ZipInfo(name + ".npy", date_time=(1980, 1, 1, 0, 0, 0))
+            info.compress_type = zipfile.ZIP_DEFLATED
+            z.writestr(info, buf.getvalue())
+
+
+def k1_edges():
+    """The reference's output for the K1 edge cases of tests/k1_cases.py (the inputs are rebuilt there, not stored)."""
+    sys.path.insert(0, os.path.join(HERE, ".."))
+    import k1_cases
+    out = {}
+    for c in k1_cases.cases():
+        name = c["name"]
+        m = TFIDF(n_gram_range=tuple(c["ngram_range"]), clean_string=c["clean"], remove_space_ngrams=c["remove_space"])
+        f, t = m._extract_tf_idf(c["frm"], c["to"], True)
+        csr_parts(name + "_from", f, out); csr_parts(name + "_to", t, out)
+        out[name + "_idf"] = m.vectorizer.idf_.astype(np.float64)
+        out[name + "_vocabulary"] = np.array(sorted(m.vectorizer.vocabulary_, key=m.vectorizer.vocabulary_.get))
+        nw, _ = m._extract_tf_idf(c["new"], c["to"], False)                 # transform with the fitted vectoriser
+        csr_parts(name + "_new", nw, out)
+        out[name + "_inputs_sha256"] = np.array(k1_cases.digest(c))
+    savez_fixed(os.path.join(HERE, "k1_edges.npz"), out)
 
 
 def main():
@@ -142,8 +178,12 @@ def main():
                                           for r in range(top_n)], 1)
         json.dump(df_to_json(df), open(os.path.join(HERE, f"dense_c1_top{top_n}.json"), "w"))
     np.savez_compressed(os.path.join(HERE, "dense_c1.npz"), **d)
+    k1_edges()
     print("golden fixtures written to", HERE)
 
 
 if __name__ == "__main__":
-    main()
+    if "--k1-edges" in sys.argv:
+        k1_edges()
+    else:
+        main()

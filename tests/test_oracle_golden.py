@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+import k1_cases
 from oracle import native, tfidf
 from oracle.assemble import assemble, cosine_topk_dense
 
@@ -238,3 +239,21 @@ def test_titles_slice_vectoriser_matches_reference(golden_dir, tag, rng, clean):
     o = tfidf.TfidfOracle(rng, clean, True).fit(list(to) + list(frm))
     np.testing.assert_array_equal(o.idf, g[tag + "_idf"])
     _eq(o.transform(frm), g, tag + "_from"); _eq(o.transform(to), g, tag + "_to")
+
+
+
+@pytest.mark.parametrize("name", k1_cases.NAMES)
+def test_k1_edges_oracles_match_reference(golden_dir, name):
+    """Rows of 255..257 and 8 191..8 192 n-gram slots, code spaces of 2^24 and just above, codes >= 2^63 (tests/k1_cases.py):
+    both oracle statements reproduce the unmodified reference's CSR, idf, vocabulary and transform bit for bit."""
+    c = k1_cases.load(golden_dir)[name]
+    g = {name + "_" + k: v for k, v in c["g"].items()}
+    rng, clean, rs = tuple(c["ngram_range"]), c["clean"], c["remove_space"]
+    f, t, vec = tfidf.fit_transform_sklearn(c["frm"], c["to"], rng, clean, rs)
+    _eq(f, g, name + "_from"); _eq(t, g, name + "_to")
+    _eq(vec.transform(c["new"]), g, name + "_new")
+    o = tfidf.TfidfOracle(rng, clean, rs).fit(c["to"] + c["frm"])
+    assert o.vocabulary == c["vocabulary"]
+    np.testing.assert_array_equal(o.idf, g[name + "_idf"])
+    _eq(o.transform(c["frm"]), g, name + "_from"); _eq(o.transform(c["to"]), g, name + "_to")
+    _eq(o.transform(c["new"]), g, name + "_new")

@@ -28,9 +28,10 @@ from polyfuzz_b200.engine import _p, _stream, _ws
 n, k = oi.shape
 for rep in range(3):
     sync(); a = time.perf_counter()
-    sims = torch.empty(k * n, dtype=torch.float64, device="cuda"); pos = torch.empty(k * n + 1, dtype=torch.int32, device="cuda")
-    bitmap = torch.empty(k * ((n + 31) // 32), dtype=torch.int32, device="cuda"); ws = _ws(_lib.load().pfz_scan_ws_bytes(k * n + 1))
-    _lib.call("pfz_frame_tail_count", _p(oi.contiguous()), _p(ov.contiguous()), n, k, _p(S.d_off), _p(sims), _p(pos), _p(bitmap), _p(ws), _stream())
+    sims = torch.empty(k * n, dtype=torch.float64, device="cuda"); pos = torch.empty(k * n + 1, dtype=torch.int64, device="cuda")
+    bitmap = torch.empty(k * ((n + 31) // 32), dtype=torch.int32, device="cuda"); ws = _ws(_lib.load().pfz_frame_tail_ws_bytes(k * n))
+    _lib.call("pfz_frame_tail_count", _p(oi.contiguous()), _p(ov.contiguous()), n, k, _p(S.d_off), _p(sims), _p(pos), _p(bitmap), _p(ws),
+              ws.numel(), _stream())
     total = int(pos[-1].item()); b = time.perf_counter()
     offsets = torch.empty(k * (n + 1), dtype=torch.int64, device="cuda"); data = torch.empty(max(total, 1), dtype=torch.uint8, device="cuda")
     _lib.call("pfz_frame_tail_copy", _p(oi.contiguous()), n, k, _p(S.d_blob), _p(S.d_off), _p(pos), _p(offsets), _p(data), _stream()); sync(); c = time.perf_counter()
