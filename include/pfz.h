@@ -100,6 +100,16 @@ int pfz_sort_u64(uint64_t *keys, int64_t n_pow2, void *stream);
 int pfz_vocab_from_sorted(const uint64_t *sorted_keys, int64_t n_keys_cap, const int64_t *n_keys_dev,
                           uint64_t *vocab_keys, int32_t *df, int32_t *n_vocab_dev, void *ws, void *stream);
 
+/* Stage B (fit), multi-GPU with a large code space.  Each rank builds its local vocabulary (sorted distinct codes V_r and
+ * their df) with the three calls above; the ranks all-gather their V_r (padded with ~0) and every rank runs pfz_sort_u64 +
+ * pfz_vocab_from_sorted on the gathered keys (n_keys = sum_r |V_r|), which yields the identical global vocabulary on every
+ * rank (the counts it returns count ranks, not documents).  Then this call stores each local code's df at its rank in that
+ * vocabulary (binary search, unsigned compare):
+ *   df[rank(local_keys[i])] = local_df[i] for i < *n_local_dev   (df: int32[n_vocab], pre-zeroed; local_cap bounds *n_local_dev)
+ * and the caller sums df across ranks (all-reduce), which gives the single-GPU df of the whole corpus.                     */
+int pfz_df_scatter(const uint64_t *local_keys, const int32_t *local_df, const int32_t *n_local_dev, int64_t local_cap,
+                   const uint64_t *vocab_keys, int32_t n_vocab, int32_t *df, void *stream);
+
 /* idf[v] = table[df[v]] for v < *n_vocab_dev: the host evaluates sklearn's np.log((n+1)/(df+1)) + 1 (sk:feature_extraction/text.py:
  * 1679-1694) once for every possible df = 0..n_docs with numpy (same bits as the reference) and the device only looks it up, so
  * neither df nor idf crosses PCIe during a fit.                                                                              */

@@ -24,6 +24,7 @@ _PROTOS = {
     "pfz_gather_codes": [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp],
     "pfz_sort_u64": [c_vp, c_i64, c_vp],
     "pfz_vocab_from_sorted": [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
+    "pfz_df_scatter": [c_vp, c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_vp],
     "pfz_idf_lookup": [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp],
     "pfz_tfidf_emit": [c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_index_build": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],

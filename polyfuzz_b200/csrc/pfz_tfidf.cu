@@ -6,7 +6,8 @@
 //
 // Stage A  ngram_rows   one warp per string: clean -> symbols -> n-gram codes -> bitonic sort -> RLE
 // Stage B  df / vocab   direct-addressed document frequency + scan compaction (small code space), or
-//                       gather + global bitonic sort + run-length (large code space)
+//                       gather + global bitonic sort + run-length (large code space); multi-GPU, large code space:
+//                       the same on the ranks' gathered vocabularies, then each rank's df scattered to global ranks
 // Stage C  emit         vocabulary lookup, tf*idf, ordered sum of squares, sqrt, divide -> CSR
 #include "pfz_common.cuh"
 
@@ -342,6 +343,18 @@ __device__ __forceinline__ int32_t lookup_col(uint64_t code, const int32_t *__re
     return (lo < n_vocab && vocab_keys[lo] == code) ? lo : -1;
 }
 
+// Multi-GPU fit, large code space: df[rank of code in the global vocabulary] = local df, for each of this rank's distinct codes.
+// A code occurs once in the local vocabulary, so no two threads store to one slot; the caller sums df across ranks.
+__global__ void df_scatter_kernel(const uint64_t *__restrict__ local_keys, const int32_t *__restrict__ local_df,
+                                  const int32_t *__restrict__ n_local, const uint64_t *__restrict__ vocab_keys, int32_t n_vocab,
+                                  int32_t *__restrict__ df) {
+    const int64_t n = *n_local;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t col = lookup_col(local_keys[i], nullptr, vocab_keys, n_vocab);
+        if (col >= 0) df[col] = local_df[i];
+    }
+}
+
 __global__ void __launch_bounds__(256) emit_count_kernel(const uint64_t *__restrict__ codes, const int64_t *__restrict__ occ_ptr,
                                                          const int32_t *__restrict__ row_cnt, int n_rows, const int32_t *__restrict__ rank_dense,
                                                          const uint64_t *__restrict__ vocab_keys, int32_t n_vocab, int32_t *__restrict__ row_nnz) {
@@ -525,6 +538,15 @@ int pfz_vocab_from_sorted(const uint64_t *sorted_keys, int64_t cap, const int64_
     sorted_compact_kernel<<<grid_for(cap, 256), 256, 0, st>>>(sorted_keys, cap, n_keys_dev, pos, vocab_keys, head_at, n_vocab_dev);
     PFZ_LAUNCH_OK();
     head_diff_kernel<<<grid_for(cap, 256), 256, 0, st>>>(head_at, n_vocab_dev, n_keys_dev, df, cap);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
+int pfz_df_scatter(const uint64_t *local_keys, const int32_t *local_df, const int32_t *n_local_dev, int64_t local_cap,
+                   const uint64_t *vocab_keys, int32_t n_vocab, int32_t *df, void *stream) {
+    PFZ_REQUIRE(local_cap >= 0 && n_vocab >= 0, "pfz_df_scatter: bad sizes (local_cap %lld, n_vocab %d)", (long long)local_cap, n_vocab);
+    if (local_cap == 0 || n_vocab == 0) return 0;
+    df_scatter_kernel<<<grid_for(local_cap, 256), 256, 0, as_stream(stream)>>>(local_keys, local_df, n_local_dev, vocab_keys, n_vocab, df);
     PFZ_LAUNCH_OK();
     return 0;
 }

@@ -5,7 +5,9 @@ The path shards by to_list row-blocks (SURVEY.md section 8e): rank r owns to-row
 GLOBAL to-indices, and the per-shard top-k lists are exchanged with ONE all-gather
 (n_from * k * 16 B per rank) followed by the pfz_topk_merge kernel with the same
 (score desc, index asc) key -- so the result is bit-identical to the single-GPU result.
-The TF-IDF fit needs the global document frequencies: one all-reduce(SUM) of the dense int32 df table.
+The TF-IDF fit needs the global vocabulary and document frequencies.  An n-gram code space of at most 2^24 takes one
+all-reduce(SUM) of the dense int32 df table.  A larger one all-gathers the ranks' sorted local vocabularies (sum_r V_r * 8 B
+received per rank), sorts the union on every rank, and all-reduces the int32 df indexed by global vocabulary rank (V * 4 B).
 """
 import torch
 import torch.distributed as dist
@@ -57,6 +59,22 @@ class Comm:
         out = torch.empty((self.world_size * n,) + tuple(local.shape[1:]), dtype=local.dtype, device=local.device)
         dist.all_gather_into_tensor(out, local, group=self.group)        # concatenated along dim 0
         return unpack_topk(out.view((self.world_size, n) + tuple(local.shape[1:])))
+
+    def all_gather_varlen(self, buf, n):
+        """Variable-length all-gather of int64 buffers: this rank contributes buf[:n] (n: an int or a one-element tensor).
+        -> (int64[G, L], [n_0, .., n_{G-1}] on the host): row r holds rank r's n_r entries followed by ~0 (-1) padding,
+        L = max(max_r n_r, 1).  Two collectives (the lengths, then the buffers padded to the longest), one host read."""
+        dev = buf.device
+        mine = torch.as_tensor(n, dtype=torch.int64, device=dev).reshape(1)
+        lens = torch.empty(self.world_size, dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(lens, mine, group=self.group)
+        lengths = [int(x) for x in lens.tolist()]
+        L = max(max(lengths), 1)
+        local = torch.full((L,), -1, dtype=torch.int64, device=dev)
+        local[:lengths[self.rank]] = buf[:lengths[self.rank]]
+        out = torch.empty((self.world_size, L), dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(out.view(-1), local, group=self.group)
+        return out, lengths
 
 
     def all_gather_best(self, idx, score, dist_):

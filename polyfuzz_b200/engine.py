@@ -165,6 +165,55 @@ class _Rows:
     __slots__ = ("n", "occ_ptr", "codes", "tf", "row_cnt", "cap", "_keep")
 
 
+def _pow2(n):
+    return 1 << max(int(n - 1).bit_length(), 1)
+
+
+def _sorted_unique(keys, n_keys, cap, d_nv):
+    """Sort `keys` (uint64 codes carried in int64, power-of-two length, ~0 after the first *n_keys) and run-length them:
+    -> (distinct codes int64[cap] ascending, multiplicities int32[cap]); *d_nv (device int32[1]) = how many."""
+    n = keys.numel()
+    _lib.call("pfz_sort_u64", _p(keys), n, _stream())
+    d_vocab = torch.empty(cap, dtype=torch.int64, device=keys.device)
+    d_cnt = torch.empty(cap, dtype=torch.int32, device=keys.device)
+    ws = _ws(n * 8 + 256 + _lib.load().pfz_scan_ws_bytes(n))
+    _lib.call("pfz_vocab_from_sorted", _p(keys), n, _p(n_keys), _p(d_vocab), _p(d_cnt), _p(d_nv), _p(ws), _stream())
+    return d_vocab, d_cnt
+
+
+def _vocab_of_rows(rows, d_nv):
+    """Vocabulary of stage-A rows for a large code space (gather + bitonic sort + run-length): (codes, df); *d_nv = V."""
+    total = sum(r.cap for r in rows)
+    keys = torch.full((_pow2(total),), -1, dtype=torch.int64, device=_dev())       # ~0 padding
+    cursor = torch.zeros(1, dtype=torch.int64, device=_dev())
+    for r in rows:
+        _lib.call("pfz_gather_codes", _p(r.codes), _p(r.occ_ptr), _p(r.row_cnt), r.n, _p(keys), _p(cursor), _stream())
+    return _sorted_unique(keys, cursor, max(total, 1), d_nv)
+
+
+def _vocab_across_ranks(rows, comm, d_nv):
+    """Multi-GPU fit with a code space too large for a dense df table.  The global vocabulary is the sorted union of the ranks'
+    local vocabularies (one variable-length all-gather, then the same sort on every rank); the global df is each rank's local
+    df stored at its codes' global ranks and summed over the ranks (one integer all-reduce).  Every rank derives the same bits
+    as a single-GPU fit of the whole corpus, and every rank raises its empty-vocabulary ValueError, after the exchange."""
+    dev = _dev()
+    loc_nv = torch.zeros(1, dtype=torch.int32, device=dev)
+    loc_vocab, loc_df = _vocab_of_rows(rows, loc_nv)
+    gathered, lengths = comm.all_gather_varlen(loc_vocab, loc_nv)              # int64[G, max V_r], ~0 padding
+    n_keys = sum(lengths)
+    keys = torch.full((_pow2(gathered.numel()),), -1, dtype=torch.int64, device=dev)
+    keys[:gathered.numel()] = gathered.reshape(-1)
+    # (the multiplicities of the union count ranks, not documents: unused)
+    d_vocab, _ = _sorted_unique(keys, torch.tensor([n_keys], dtype=torch.int64, device=dev), max(n_keys, 1), d_nv)
+    V = int(d_nv.item())
+    if V == 0:
+        raise ValueError("empty vocabulary; perhaps the documents only contain stop words")
+    d_df = torch.zeros(V, dtype=torch.int32, device=dev)
+    _lib.call("pfz_df_scatter", _p(loc_vocab), _p(loc_df), _p(loc_nv), int(loc_vocab.numel()), _p(d_vocab), V, _p(d_df), _stream())
+    comm.all_reduce_sum(d_df)
+    return d_vocab, d_df
+
+
 class NgramTfidf:
     """GPU statement of `TfidfVectorizer(min_df=1, analyzer=TFIDF._create_ngrams)` as the reference
     uses it (polyfuzz/models/_tfidf.py:102-118).  fit() learns vocabulary (alphabetical == ascending
@@ -294,7 +343,8 @@ class NgramTfidf:
         """Fit on device-resident lists.  Multi-GPU (comm given): `counted[i]` says whether list i
         contributes to df / n_docs on THIS rank (a replicated list is counted on rank 0 only); the
         dense df table and the document count are summed across ranks (one all-reduce), after which
-        every rank derives the identical vocabulary and idf."""
+        every rank derives the identical vocabulary and idf.  A code space above DENSE_CODE_SPACE_MAX
+        all-gathers the ranks' local vocabularies instead (_vocab_across_ranks)."""
         if counted is None:
             counted = [True] * len(staged)
         if not self.clean:
@@ -310,11 +360,10 @@ class NgramTfidf:
         cs = self.code_space()
         total_cap = sum(r.cap for r in rows)
         if comm is not None:
-            if cs > DENSE_CODE_SPACE_MAX:
-                raise NotImplementedError("multi-GPU fit needs an n-gram code space <= 2^24 (e.g. cleaned n <= 4)")
             if n_docs_total is not None:
                 # the caller knows the global document count (every rank sees the list lengths): no collective, no host sync here;
-                # the vocabulary buffers are then sized by the code space instead of the summed n-gram slots
+                # the dense vocabulary buffers are then sized by the code space instead of the summed n-gram slots (the large
+                # code space path sizes its buffers from the gathered vocabulary lengths)
                 n_docs, total_cap_all = int(n_docs_total), cs
             else:
                 meta = torch.tensor([n_docs, total_cap], dtype=torch.int64, device=dev)
@@ -337,18 +386,12 @@ class NgramTfidf:
             d_rank = torch.empty(cs, dtype=torch.int32, device=dev)
             ws = _ws(_lib.load().pfz_scan_ws_bytes(cs))
             _lib.call("pfz_vocab_compact_dense", _p(df_dense), cs, _p(d_vocab), _p(d_df), _p(d_rank), _p(d_nv), _p(ws), _stream())
-        else:
-            cap2 = 1 << max(int(total_cap - 1).bit_length(), 1)
-            keys = torch.full((cap2,), -1, dtype=torch.int64, device=dev)       # ~0 padding
-            cursor = torch.zeros(1, dtype=torch.int64, device=dev)
-            for r in rows:
-                _lib.call("pfz_gather_codes", _p(r.codes), _p(r.occ_ptr), _p(r.row_cnt), r.n, _p(keys), _p(cursor), _stream())
-            _lib.call("pfz_sort_u64", _p(keys), cap2, _stream())
-            d_vocab = torch.empty(total_cap, dtype=torch.int64, device=dev)
-            d_df = torch.empty(total_cap, dtype=torch.int32, device=dev)
+        elif comm is not None:
+            d_vocab, d_df = _vocab_across_ranks([r for r, c in zip(rows, counted) if c], comm, d_nv)
             d_rank = None
-            ws = _ws(cap2 * 8 + 256 + _lib.load().pfz_scan_ws_bytes(cap2))
-            _lib.call("pfz_vocab_from_sorted", _p(keys), cap2, _p(cursor), _p(d_vocab), _p(d_df), _p(d_nv), _p(ws), _stream())
+        else:
+            d_vocab, d_df = _vocab_of_rows(rows, d_nv)
+            d_rank = None
         # idf exactly as scikit-learn computes it on the host (sk:feature_extraction/text.py:1679-1694):
         # np.log((n_samples + 1) / (df + 1)) + 1 -- same numpy, same bits as the reference on this machine -- as a TABLE over
         # every possible df (0..n_docs), looked up on the device: no df D2H, no idf H2D, nothing waits for the host.
