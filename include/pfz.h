@@ -468,6 +468,29 @@ int pfz_frame_tail_count(const int32_t *top_idx, const double *top_val, int32_t 
 int pfz_frame_tail_copy(const int32_t *top_idx, int32_t n, int32_t k, const int32_t *to_blob, const int64_t *to_offsets, const int64_t *pos,
                         int64_t *offsets, uint8_t *data, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * K6  word-vector lookup and mean pooling (csrc/pfz_wordvec.cu).
+ * Replaces: GensimEmbeddings._embed, polyfuzz/models/_gensim.py:118-140 (s.split(" "), kv.get_vector or np.zeros(d) on
+ *           KeyError, np.mean(axis=0), np.array of the rows).  DESIGN.md 4.11 states the contract.
+ * The vocabulary: keys as code points (key_blob uint32, key_off int64[n_keys+1], distinct), key_row int32[n_keys] = the row of
+ * V each key maps to (kv.key_to_index[key]), V float32 or float64 [n_rows][d] row-major, d >= 2.
+ *
+ * pfz_wv_table_build: open-addressing hash table over the keys, table int32[cap] (cap a power of two > n_keys, <= 2^31; -1 =
+ *   empty slot, else a key's position in the key list), filled by atomicCAS inserts with linear probing.
+ * pfz_wv_lookup: each string split on U+0020 only (s spaces give s + 1 tokens, empty tokens included); tok_off int64[n+1]
+ *   receives the token offsets (a device scan), tok_row int32[>= n_chars + n] the row of V of each token, or -1 when no key
+ *   equals it (equal length and code points).  ws: ws_bytes >= pfz_wv_lookup_ws_bytes(n).  No host synchronisation.
+ * pfz_wv_pool: out float64 [n][ld] (ld >= d) = the mean of each string's token rows, bit for bit numpy's: in float32 when V is
+ *   float32 and every token of the string was found (sequential sum, then the quotient rounded to float32), in float64
+ *   otherwise (missing tokens add +0.0; the first token's value starts the sum).                                             */
+int pfz_wv_table_build(const uint32_t *key_blob, const int64_t *key_off, int32_t n_keys, int32_t *table, int64_t cap, void *stream);
+int64_t pfz_wv_lookup_ws_bytes(int32_t n);
+int pfz_wv_lookup(const uint32_t *blob, const int64_t *offsets, int32_t n, const uint32_t *key_blob, const int64_t *key_off,
+                  const int32_t *key_row, const int32_t *table, int64_t cap, int64_t *tok_off, int32_t *tok_row, void *ws, int64_t ws_bytes,
+                  void *stream);
+int pfz_wv_pool(const void *vectors, int32_t is_f64, int32_t d, const int64_t *tok_off, const int32_t *tok_row, int32_t n, double *out,
+                int64_t ld, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,6 +1,6 @@
 """polyfuzz_b200 -- H100-native (sm_90a) pairwise string-similarity hot path behind PolyFuzz's
 BaseMatcher plugin API.  See DESIGN.md / INTEGRATION.md."""
-from .matchers import BaseMatcher, TFIDF, RapidFuzz, EditDistance, Embeddings  # noqa: F401
+from .matchers import BaseMatcher, TFIDF, RapidFuzz, EditDistance, Embeddings, GensimEmbeddings  # noqa: F401
 
 __version__ = "0.1.0"
 

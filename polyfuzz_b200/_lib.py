@@ -70,10 +70,15 @@ _PROTOS = {
     "pfz_dense_cos_cand_f16": [c_vp, c_vp, c_i32, c_i32, c_i32, c_f64, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp],
     "pfz_dense_topn_exact_rescore": [c_vp, c_vp, c_i32, c_i32, c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp],
     "pfz_dense_topn_select": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp],
+    "pfz_wv_table_build": [c_vp, c_vp, c_i32, c_vp, c_i64, c_vp],
+    "pfz_wv_lookup_ws_bytes": [c_i32],
+    "pfz_wv_lookup": [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp],
+    "pfz_wv_pool": [c_vp, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64, c_vp],
 }
 _RESTYPES = {"pfz_last_error": ctypes.c_char_p, "pfz_scan_ws_bytes": c_i64, "pfz_launch_count": c_i64, "pfz_spcos_block_ws_bytes": c_i64,
              "pfz_spcos_block_gcnt_offset": c_i64,
-             "pfz_dense_exact_fallback_ws_bytes": c_i64, "pfz_frame_tail_ws_bytes": c_i64}
+             "pfz_dense_exact_fallback_ws_bytes": c_i64, "pfz_frame_tail_ws_bytes": c_i64,
+             "pfz_wv_lookup_ws_bytes": c_i64}
 
 
 def exported_names():
