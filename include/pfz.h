@@ -491,6 +491,21 @@ int pfz_wv_lookup(const uint32_t *blob, const int64_t *offsets, int32_t n, const
 int pfz_wv_pool(const void *vectors, int32_t is_f64, int32_t d, const int64_t *tok_off, const int32_t *tok_row, int32_t n, double *out,
                 int64_t ld, void *stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * K7  single linkage (csrc/pfz_linkage.cu).
+ * Replaces: polyfuzz/linkage.py:25-51 (the kept rows' dict loop and the clusters / cluster_name_map built from it).  DESIGN.md
+ *           4.13 states the rule.  Rows: int32 key ids F[n], T[n] in [0, n_keys); a row is kept when similarity is NULL or
+ *           similarity[p] > min_similarity (NaN is not kept).  n < 2^30.
+ * Outputs, per key (int32[n_keys]): val = its final value in cluster_mapping (-1 when never written), rank = its position in
+ *   cluster_mapping's insertion order (-1 when never written), rep = the key cluster_name_map maps it to (-1 when never
+ *   written); grouped = the written keys in the order of the reference's `clusters` (clusters by their first key, each in
+ *   insertion order; -1 past the written keys); n_written int32[1] = the number of keys written.
+ * ws: ws_bytes >= pfz_linkage_ws_bytes(n, n_keys) (-1 on error).  No host synchronisation: a fixed number of rounds and pointer
+ *   jumps are enqueued, each returning at once when nothing is left, and a one-warp kernel finishes what the rounds leave. */
+int64_t pfz_linkage_ws_bytes(int32_t n, int32_t n_keys);
+int pfz_linkage(const int32_t *F, const int32_t *T, int32_t n, const double *similarity, double min_similarity, int32_t n_keys,
+                int32_t *val, int32_t *rank, int32_t *rep, int32_t *grouped, int32_t *n_written, void *ws, int64_t ws_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

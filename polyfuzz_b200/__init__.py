@@ -1,6 +1,7 @@
 """polyfuzz_b200 -- H100-native (sm_90a) pairwise string-similarity hot path behind PolyFuzz's
 BaseMatcher plugin API.  See DESIGN.md / INTEGRATION.md."""
 from .matchers import BaseMatcher, TFIDF, RapidFuzz, EditDistance, Embeddings, GensimEmbeddings  # noqa: F401
+from .linkage import single_linkage, install_linkage  # noqa: F401
 
 __version__ = "0.1.0"
 

@@ -74,11 +74,13 @@ _PROTOS = {
     "pfz_wv_lookup_ws_bytes": [c_i32],
     "pfz_wv_lookup": [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp],
     "pfz_wv_pool": [c_vp, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64, c_vp],
+    "pfz_linkage_ws_bytes": [c_i32, c_i32],
+    "pfz_linkage": [c_vp, c_vp, c_i32, c_vp, c_f64, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp],
 }
 _RESTYPES = {"pfz_last_error": ctypes.c_char_p, "pfz_scan_ws_bytes": c_i64, "pfz_launch_count": c_i64, "pfz_spcos_block_ws_bytes": c_i64,
              "pfz_spcos_block_gcnt_offset": c_i64,
              "pfz_dense_exact_fallback_ws_bytes": c_i64, "pfz_frame_tail_ws_bytes": c_i64,
-             "pfz_wv_lookup_ws_bytes": c_i64}
+             "pfz_wv_lookup_ws_bytes": c_i64, "pfz_linkage_ws_bytes": c_i64}
 
 
 def exported_names():
