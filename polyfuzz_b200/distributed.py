@@ -5,6 +5,7 @@ The path shards by to_list row-blocks (SURVEY.md section 8e): rank r owns to-row
 GLOBAL to-indices, and the per-shard top-k lists are exchanged with ONE all-gather
 (n_from * k * 16 B per rank) followed by the pfz_topk_merge kernel with the same
 (score desc, index asc) key -- so the result is bit-identical to the single-GPU result.
+tfidf_topk_sharded drives TF-IDF on one GPU too (comm=None: one shard, no collectives).
 The TF-IDF fit needs the global vocabulary and document frequencies.  An n-gram code space of at most 2^24 takes one
 all-reduce(SUM) of the dense int32 df table.  A larger one all-gathers the ranks' sorted local vocabularies (sum_r V_r * 8 B
 received per rank), sorts the union on every rank, and all-reduces the int32 df indexed by global vocabulary rank (V * 4 B).
@@ -155,7 +156,11 @@ def get_comm(group=None):
 def tfidf_topk_sharded(vectorizer, staged_from, staged_to_shard, to_index_base, top_n, min_similarity,
                        self_match, from_index_base=0, fit=True, fit_on_from=True, comm=None, index=None,
                        tile=None, timings=None, k1_timings=None, n_docs_total=None):
-    """Sharded TF-IDF top-k.  Every rank passes the same from-list and its own to-shard.
+    """TF-IDF top-k: K1, the K2 index (engine.index_for) and K2 -- the one driver of TFIDF.match, on one GPU (comm=None,
+    the to-list is one shard at base 0) and on many.  Every rank passes the same from-list and its own to-shard; a
+    single-GPU self-match passes the same StagedStrings as both, and one matrix serves both sides.
+    fit=False transforms with the fitted vectoriser against `index`, which is replaced when the new from-rows are too long
+    for its kernel; staged_from may then be an already vectorised from-matrix (engine.CsrMatrix).
     n_docs_total: the number of documents the fit counts over ALL ranks (to-rows of every shard + the from-list when
     fit_on_from), when the caller knows it -- saves one small all-reduce and a host sync per fit.
     Returns (top_idx[n_from,k] GLOBAL indices, top_val[n_from,k], csr_to_shard, index)."""
@@ -174,15 +179,15 @@ def tfidf_topk_sharded(vectorizer, staged_from, staged_to_shard, to_index_base, 
         else:
             rows_to, rows_from = vectorizer.fit_staged(staged, counted=counted, comm=comm, n_docs_total=n_docs_total)
         csr_to = vectorizer.emit(rows_to)
-        index = engine.SparseIndex(csr_to, tile=tile, variant=engine.choose_variant(vectorizer.density(), vectorizer.max_row_nnz, csr_to.n_rows))
+        index = engine.index_for(csr_to, vectorizer, tile=tile)
         csr_from = csr_to if same else vectorizer.emit(rows_from)
     else:
         csr_to = None
-        csr_from = vectorizer.emit(vectorizer.rows(staged_from))
-        if index.variant in ("dense32", "block") and vectorizer.max_row_nnz > engine.DENSE32_MAX_ROW_NNZ:
-            index = engine.SparseIndex(index.csr, tile=tile, variant="dense")
-        elif index.variant == "hash" and vectorizer.max_row_nnz > engine.HASH_MAX_ROW_NNZ:
-            index = engine.SparseIndex(index.csr, tile=tile, variant="list")
+        if isinstance(staged_from, engine.CsrMatrix):       # already vectorised (a self-match transform on one GPU)
+            csr_from = staged_from
+        else:
+            csr_from = vectorizer.emit(vectorizer.rows(staged_from))
+        index = engine.index_for(index.csr, vectorizer, index, tile)
     if ev1 is not None:
         ev1[1].record()
         k1_timings.append(ev1)

@@ -5,7 +5,9 @@ Classes
     NgramTfidf   K1: fit / transform of the char-n-gram TF-IDF vectoriser -> CSR tensors in HBM
     SparseIndex  inverted index of a to-matrix (term x to-tile posting segments)
 Functions
+    index_for    the K2 index of a TF-IDF to-matrix: picks the variant, and replaces it when from-rows outgrow its kernel
     spcos_topk   K2: fused sparse cosine + per-row top-k (pages of 32 for larger k), tile splits + merge
+The TF-IDF path K1 -> index -> K2 is driven by distributed.tfidf_topk_sharded, on one GPU and on many.
 """
 import ctypes
 import os
@@ -340,8 +342,9 @@ class NgramTfidf:
         return self.fit_staged([self.stage(l) for l in lists])
 
     def fit_staged(self, staged, counted=None, comm=None, n_docs_total=None):
-        """Fit on device-resident lists.  Multi-GPU (comm given): `counted[i]` says whether list i
-        contributes to df / n_docs on THIS rank (a replicated list is counted on rank 0 only); the
+        """Fit on device-resident lists.  `counted[i]` says whether list i contributes to the vocabulary, df and
+        n_docs (on THIS rank): a list that is only scored, such as a from-block of a self-match, is not counted, and a
+        list replicated on every rank is counted on rank 0 only.  Multi-GPU (comm given): the
         dense df table and the document count are summed across ranks (one all-reduce), after which
         every rank derives the identical vocabulary and idf.  A code space above DENSE_CODE_SPACE_MAX
         all-gathers the ranks' local vocabularies instead (_vocab_across_ranks)."""
@@ -354,7 +357,8 @@ class NgramTfidf:
             raise ValueError(f"alphabet of {self.base - 1} symbols with {self.hi}-grams exceeds 64-bit n-gram codes")
         d_sym = self._sym_table()
         rows = [self._stage_a(S, d_sym, fit=True) for S in staged]
-        n_docs = sum(r.n for r, c in zip(rows, counted) if c)
+        counted_rows = [r for r, c in zip(rows, counted) if c]
+        n_docs = sum(r.n for r in counted_rows)
         dev = _dev()
         d_nv = torch.zeros(1, dtype=torch.int32, device=dev)
         cs = self.code_space()
@@ -375,9 +379,8 @@ class NgramTfidf:
             raise ValueError("empty vocabulary; perhaps the documents only contain stop words")
         if cs <= DENSE_CODE_SPACE_MAX:
             df_dense = torch.zeros(cs, dtype=torch.int32, device=dev)
-            for r, c in zip(rows, counted):
-                if c:
-                    _lib.call("pfz_df_dense", _p(r.codes), _p(r.occ_ptr), _p(r.row_cnt), r.n, _p(df_dense), _stream())
+            for r in counted_rows:
+                _lib.call("pfz_df_dense", _p(r.codes), _p(r.occ_ptr), _p(r.row_cnt), r.n, _p(df_dense), _stream())
             if comm is not None:
                 comm.all_reduce_sum(df_dense)
             vmax = min(cs, total_cap_all)
@@ -387,10 +390,10 @@ class NgramTfidf:
             ws = _ws(_lib.load().pfz_scan_ws_bytes(cs))
             _lib.call("pfz_vocab_compact_dense", _p(df_dense), cs, _p(d_vocab), _p(d_df), _p(d_rank), _p(d_nv), _p(ws), _stream())
         elif comm is not None:
-            d_vocab, d_df = _vocab_across_ranks([r for r, c in zip(rows, counted) if c], comm, d_nv)
+            d_vocab, d_df = _vocab_across_ranks(counted_rows, comm, d_nv)
             d_rank = None
         else:
-            d_vocab, d_df = _vocab_of_rows(rows, d_nv)
+            d_vocab, d_df = _vocab_of_rows(counted_rows, d_nv)
             d_rank = None
         # idf exactly as scikit-learn computes it on the host (sk:feature_extraction/text.py:1679-1694):
         # np.log((n_samples + 1) / (df + 1)) + 1 -- same numpy, same bits as the reference on this machine -- as a TABLE over
@@ -542,6 +545,20 @@ def choose_variant(density, max_row_nnz=None, n_to=None):
     if DENSE_VARIANT in ("dense32", "block") and (max_row_nnz is None or max_row_nnz > DENSE32_MAX_ROW_NNZ):
         return "dense"
     return DENSE_VARIANT
+
+
+def index_for(csr_to, vec, index=None, tile=None):
+    """The K2 index of the TF-IDF to-matrix csr_to for from-rows of up to vec.max_row_nnz terms.
+    index=None: a new index of the variant choose_variant picks for the fitted vectoriser vec.  Otherwise `index` itself
+    while its kernel takes rows that long; if not, a new index on index.csr for the fp64 kernel of the same regime: the
+    block (and dense32) kernel holds 128 terms per row, the hash kernel 256, and both only flag a longer row on the device."""
+    if index is None:
+        return SparseIndex(csr_to, tile, variant=choose_variant(vec.density(), vec.max_row_nnz, csr_to.n_rows))
+    if index.variant in ("dense32", "block") and vec.max_row_nnz > DENSE32_MAX_ROW_NNZ:
+        return SparseIndex(index.csr, tile, variant="dense")
+    if index.variant == "hash" and vec.max_row_nnz > HASH_MAX_ROW_NNZ:
+        return SparseIndex(index.csr, tile, variant="list")
+    return index
 
 
 def _auto_splits(n_from, n_tiles, sm_count=132):

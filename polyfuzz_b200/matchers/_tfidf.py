@@ -1,5 +1,6 @@
 """TFIDF matcher -- drop-in for polyfuzz.models.TFIDF (polyfuzz/models/_tfidf.py:11-146) running the
-vectoriser (K1) and the sparse cosine top-n (K2) on an H100."""
+vectoriser (K1) and the sparse cosine top-n (K2) on an H100, on one GPU or many through the same driver
+(distributed.tfidf_topk_sharded)."""
 from typing import List, Tuple
 
 import numpy as np
@@ -57,7 +58,7 @@ class TFIDF(BaseMatcher):
         self.remove_space_ngrams = remove_space_ngrams
         self.distributed = distributed
         self._index = None              # device inverted index of tf_idf_to (rebuilt lazily after unpickling)
-        self._shard = (0, 0)            # distributed: [lo, hi) to-rows owned by this rank
+        self._shard = (0, 0)            # [lo, hi) to-rows owned by this rank (all of them on one GPU)
         self._st_to = None              # device-resident to-list (blob, offsets) for the frame tail; not pickled
         self._st_from = None            # ... and the from-rows of the current call
 
@@ -101,113 +102,56 @@ class TFIDF(BaseMatcher):
         return self.min_similarity
 
     def match_arrays(self, from_list, to_list=None, re_train=True, from_block=None):
-        """Device-side result: (top_idx int32[n,k] with -1 for no match, top_val float64[n,k], k)."""
+        """Device-side result: (top_idx int32[n,k] with -1 for no match, top_val float64[n,k], k).
+        One GPU or many, the lists are staged here and scored by one driver (distributed.tfidf_topk_sharded)."""
         top_n = clip_top_n(self.top_n, to_list)
         if top_n < 1:
             raise ValueError("top_n must be >= 1 and to_list must not be empty")
+        from_base, rows = 0, from_list
         if from_block is not None:
             if to_list is not None:
                 raise ValueError("from_block is only meaningful for a self-match (to_list=None)")
             lo, hi = int(from_block[0]), int(from_block[1])
             if not (0 <= lo <= hi <= len(from_list)):
                 raise ValueError(f"from_block {from_block} out of range")
-        comm = get_comm() if self.distributed else None
-        if comm is not None:
-            return self._match_sharded(comm, from_list, to_list, re_train, top_n, from_block) + (top_n,)
-        if from_block is not None:
-            # fit / index on the whole list, score only the block's rows (global diagonal excluded)
-            self._extract_tf_idf(from_list, None, re_train)
-            block_rows = self.vectorizer.rows(from_list[lo:hi])
-            self._st_from = block_rows._keep
-            block = self.vectorizer.emit(block_rows)
-            idx, val = engine.spcos_topk(block, self._safe_index(), top_n, self._threshold(), self_match=True,
-                                         from_index_base=lo)
-            return idx, val, top_n
-        tf_idf_from, tf_idf_to = self._extract_tf_idf(from_list, to_list, re_train)
-        idx, val = engine.spcos_topk(tf_idf_from, self._safe_index(), top_n, self._threshold(),
-                                     self_match=to_list is None)
-        return idx, val, top_n
-
-    def _extract_tf_idf(self, from_list, to_list=None, re_train=True):
-        """polyfuzz/models/_tfidf.py:102-118 (note `if to_list:` -- an empty list means self-match for the
-        vectoriser while `cosine_similarity` still tests `is not None`)."""
-        if re_train:
-            self.vectorizer = engine.NgramTfidf(self.n_gram_range, self.clean_string, self.remove_space_ngrams)
-        elif self.vectorizer is None:
-            raise ValueError("re_train=False needs a fitted model (call match/fit first)")
-        vec = self.vectorizer
-        if to_list:
-            if re_train:
-                rows_to, rows_from = vec.fit_rows([to_list, from_list])
-                self.tf_idf_to = vec.emit(rows_to)
-                self._index = None
-                self._st_to = self._tail_of(rows_to._keep)
-            else:
-                rows_from = vec.rows(from_list)
-            self._st_from = rows_from._keep
-            tf_idf_from = vec.emit(rows_from)
-        else:
-            if re_train:
-                (rows_from,) = vec.fit_rows([from_list])
-                self.tf_idf_to = vec.emit(rows_from)
-                self._index = None
-                self._st_to = self._tail_of(rows_from._keep)
-                self._st_from = rows_from._keep
-            elif self._st_to is not None:
-                self._st_from = self._st_to[3]
-            tf_idf_from = self._device_to()
-        if self._index is None:
-            self._index = engine.SparseIndex(self._device_to(), variant=engine.choose_variant(vec.density(), vec.max_row_nnz, self._device_to().n_rows))
-        return tf_idf_from, self.tf_idf_to
-
-    @staticmethod
-    def _tail_of(S):
-        """(device blob int32, device offsets int64, ascii?, staged list) of a to-list kept for the frame tail (K5)."""
-        return (S.d_blob, S.d_off, bool(S.ascii), S)
-
-    def _match_sharded(self, comm, from_list, to_list, re_train, top_n, from_block=None):
+            from_base, rows = lo, from_list[lo:hi]
+        threshold = self._threshold()
         if re_train:
             self.vectorizer = engine.NgramTfidf(self.n_gram_range, self.clean_string, self.remove_space_ngrams)
         elif self.vectorizer is None or self.tf_idf_to is None:
             raise ValueError("re_train=False needs a fitted model (call match/fit first)")
         vec = self.vectorizer
-        if not re_train and self._index is None:             # restored from a pickle: the shard's index is rebuilt from its CSR
-            self._index = engine.SparseIndex(self._device_to(), variant=engine.choose_variant(vec.density(), vec.max_row_nnz, self._device_to().n_rows))
-        self_match = to_list is None
+        comm = get_comm() if self.distributed else None
         full_to = to_list if to_list else from_list          # `if to_list:` as in _tfidf.py:107
-        from_base = 0
-        if from_block is not None:
-            from_base = int(from_block[0])
-            from_list = from_list[from_block[0]:from_block[1]]
-        staged_from = vec.stage(from_list)
-        self._st_from = staged_from
+        staged_to = None
         if re_train:
-            lo, hi = shard_bounds(len(full_to), comm.world_size, comm.rank)
-            self._shard = (lo, hi)
-            staged_to = vec.stage(full_to[lo:hi])
+            self._shard = shard_bounds(len(full_to), comm.world_size, comm.rank) if comm else (0, len(full_to))
+            lo, hi = self._shard
+            staged_to = vec.stage(full_to[lo:hi] if comm else full_to)
             # the frame tail needs every to-string on every rank: the shards' blobs are all-gathered over NCCL (bytes), so the
             # host work per rank stays that of its own shard
-            self._st_to = gather_string_shards(comm, staged_to)
+            self._st_to = gather_string_shards(comm, staged_to) if comm else self._tail_of(staged_to)
+        if comm is None and not to_list and from_block is None:
+            # one GPU, whole self-match: the to-list is the from-list (polyfuzz/models/_tfidf.py:114-116); a transform
+            # scores the fitted to-matrix itself instead of vectorising the list again
+            staged_from = staged_to if re_train else self._device_to()
+            self._st_from = staged_to if re_train else (self._st_to[3] if self._st_to is not None else None)
         else:
-            lo, hi = self._shard
-            staged_to = None
-        idx, val, csr_to, index = tfidf_topk_sharded(vec, staged_from, staged_to, lo, top_n, self._threshold(),
-                                                     self_match, from_base, fit=re_train, fit_on_from=bool(to_list), comm=comm,
-                                                     index=self._index,
-                                                     n_docs_total=len(full_to) + (len(from_list) if to_list else 0))
+            staged_from = self._st_from = vec.stage(rows)
+        if not re_train and self._index is None:             # restored from a pickle: the index is rebuilt from the to-matrix
+            self._index = engine.index_for(self._device_to(), vec)
+        idx, val, csr_to, self._index = tfidf_topk_sharded(vec, staged_from, staged_to, self._shard[0], top_n, threshold,
+                                                           to_list is None, from_base, fit=re_train, fit_on_from=bool(to_list),
+                                                           comm=comm, index=self._index,
+                                                           n_docs_total=len(full_to) + (len(from_list) if to_list else 0))
         if re_train:
             self.tf_idf_to = csr_to
-        self._index = index                                  # also when a transform had to fall back to the fp64 kernel
-        return idx, val
+        return idx, val, top_n
 
-    def _safe_index(self):
-        """A later transform() may bring from-rows longer than the mixed-precision bound allows: rebuild the
-        index for the fp64 kernel then (the to-matrix is unchanged)."""
-        if self._index.variant in ("dense32", "block") and self.vectorizer.max_row_nnz > engine.DENSE32_MAX_ROW_NNZ:
-            self._index = engine.SparseIndex(self._device_to(), variant="dense")
-        elif self._index.variant == "hash" and self.vectorizer.max_row_nnz > engine.HASH_MAX_ROW_NNZ:
-            self._index = engine.SparseIndex(self._device_to(), variant="list")
-        return self._index
+    @staticmethod
+    def _tail_of(S):
+        """(device blob int32, device offsets int64, ascii?, staged list) of a to-list kept for the frame tail (K5)."""
+        return (S.d_blob, S.d_off, bool(S.ascii), S)
 
     def _device_to(self):
         if hasattr(self.tf_idf_to, "tocsr"):                      # restored from a pickle

@@ -116,7 +116,7 @@ def single(frm, to, rng, clean, k, from_block=None):
 
 
 def sharded(comm, frm, to, rng, clean, k, from_block=None, n_docs_total=True):
-    """What TFIDF._match_sharded does on one rank, without the string exchange of the frame tail."""
+    """What TFIDF.match_arrays does on one rank, without the string exchange of the frame tail."""
     from polyfuzz_b200 import engine
     from polyfuzz_b200.distributed import shard_bounds, tfidf_topk_sharded
     v = engine.NgramTfidf(rng, clean, True)

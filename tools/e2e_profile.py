@@ -14,7 +14,7 @@ for rep in range(5):
     S = vec.stage(names); sync(); t1 = time.perf_counter(); T["stage(pack+H2D)"] = t1 - t0
     (rows,) = vec.fit_staged([S]); sync(); t2 = time.perf_counter(); T["fit"] = t2 - t1
     csr = vec.emit(rows); sync(); t3 = time.perf_counter(); T["emit"] = t3 - t2
-    ix = engine.SparseIndex(csr, variant=engine.choose_variant(vec.density(), vec.max_row_nnz, csr.n_rows)); sync(); t4 = time.perf_counter(); T["index"] = t4 - t3
+    ix = engine.index_for(csr, vec); sync(); t4 = time.perf_counter(); T["index"] = t4 - t3
     oi, ov = engine.spcos_topk(csr, ix, 10, 0.0, self_match=True); sync(); t5 = time.perf_counter(); T["K2 " + ix.variant] = t5 - t4
     fa = U.arrow_from_staged(S); t6 = time.perf_counter(); T["from arrow"] = t6 - t5
     df = U.assemble_matches_device(fa, S.d_blob, S.d_off, oi, ov); t7 = time.perf_counter(); T["tail K5 + D2H + wrap"] = t7 - t6
