@@ -490,6 +490,15 @@ int pfz_wv_lookup(const uint32_t *blob, const int64_t *offsets, int32_t n, const
                   void *stream);
 int pfz_wv_pool(const void *vectors, int32_t is_f64, int32_t d, const int64_t *tok_off, const int32_t *tok_row, int32_t n, double *out,
                 int64_t ld, void *stream);
+/* pfz_ft_pool: the same out as pfz_wv_pool for a FastText model with bucket > 0.
+ * Replaces: polyfuzz/models/_gensim.py:128-136 with kv a gensim FastTextKeyedVectors, whose get_vector(word) builds a word
+ *   outside the vocabulary from its character n-grams.  DESIGN.md 4.14 states the contract.
+ * blob/offsets: the strings given to pfz_wv_lookup, and its tok_off / tok_row.  vectors float32 [n_rows][d], vectors_ngrams
+ *   float32 [>= bucket][d], 1 <= bucket < 2^32, min_n, max_n >= 0; no code point of the strings is a surrogate.  A token with
+ *   tok_row -1 is the float32 mean of the rows h % bucket of the n-grams of "<" + token + ">" (h: 32-bit FNV-1a over the UTF-8
+ *   bytes, each sign-extended), +0.0 without n-grams; every string is then pooled in float32.  No host synchronisation.     */
+int pfz_ft_pool(const uint32_t *blob, const int64_t *offsets, int32_t n, const int64_t *tok_off, const int32_t *tok_row, const float *vectors,
+                const float *vectors_ngrams, int32_t d, int64_t bucket, int32_t min_n, int32_t max_n, double *out, int64_t ld, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K7  single linkage (csrc/pfz_linkage.cu).

@@ -74,6 +74,7 @@ _PROTOS = {
     "pfz_wv_lookup_ws_bytes": [c_i32],
     "pfz_wv_lookup": [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp],
     "pfz_wv_pool": [c_vp, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_i64, c_vp],
+    "pfz_ft_pool": [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp],
     "pfz_linkage_ws_bytes": [c_i32, c_i32],
     "pfz_linkage": [c_vp, c_vp, c_i32, c_vp, c_f64, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp],
 }

@@ -9,6 +9,8 @@
 //                table, comparing the full code-point sequence of every key whose slot it meets
 //   pool         one warp per string, lanes over columns: numpy's sequential axis-0 sum in the dtype of the token list, and
 //                one division by the token count (DESIGN.md 4.11 states the rule)
+//   FastText     pfz_ft_pool: the pool with every token in float32, a token missing from the vocabulary replaced by gensim's
+//                subword vector, hashed and gathered in place by the string's warp (DESIGN.md 4.14)
 #include <cub/device/device_scan.cuh>
 #include "pfz_common.cuh"
 
@@ -151,6 +153,134 @@ __global__ void __launch_bounds__(WV_THREADS) wv_pool_kernel(const T *__restrict
     }
 }
 
+// ---- FastText subword vectors (DESIGN.md 4.14) ------------------------------------------------------------------------------------
+// gensim's FastTextKeyedVectors.get_vector(word) for a word outside the vocabulary: the n-grams of "<" + word + ">" (characters,
+// i ascending, n = 1..max_n ascending, kept when n >= min_n and not the lone "<" or ">"), each hashed by 32-bit FNV-1a over its
+// UTF-8 bytes sign-extended, bucket = h % bucket; the vector is fl32(sum) / count in float32, +0.0 without n-grams.
+constexpr int FT_COLS = 10;         // columns per lane in one pass of the FastText pool kernel: 320 columns, d = 300 in one pass
+
+// character k of "<" + tok[0..len) + ">"
+__device__ __forceinline__ uint32_t ft_char(const uint32_t *__restrict__ tok, int64_t len, int64_t k) {
+    return k == 0 ? 60u : k == len + 1 ? 62u : tok[k - 1];
+}
+
+__device__ __forceinline__ uint32_t ft_fnv_byte(uint32_t h, uint32_t b) {
+    return (h ^ (b >= 0x80u ? 0xFFFFFF00u | b : b)) * 16777619u;      // the byte as int8, sign-extended to 32 bits
+}
+
+// FNV-1a over the UTF-8 encoding of characters [i, i + n) of "<" + tok + ">" (no surrogates: the host refuses them)
+__device__ __forceinline__ uint32_t ft_hash(const uint32_t *__restrict__ tok, int64_t len, int64_t i, int64_t n) {
+    uint32_t h = 2166136261u;
+    for (int64_t k = i; k < i + n; ++k) {
+        const uint32_t c = ft_char(tok, len, k);
+        if (c < 0x80u) {
+            h = ft_fnv_byte(h, c);
+        } else if (c < 0x800u) {
+            h = ft_fnv_byte(h, 0xC0u | (c >> 6));
+            h = ft_fnv_byte(h, 0x80u | (c & 0x3Fu));
+        } else if (c < 0x10000u) {
+            h = ft_fnv_byte(h, 0xE0u | (c >> 12));
+            h = ft_fnv_byte(h, 0x80u | ((c >> 6) & 0x3Fu));
+            h = ft_fnv_byte(h, 0x80u | (c & 0x3Fu));
+        } else {
+            h = ft_fnv_byte(h, 0xF0u | (c >> 18));
+            h = ft_fnv_byte(h, 0x80u | ((c >> 12) & 0x3Fu));
+            h = ft_fnv_byte(h, 0x80u | ((c >> 6) & 0x3Fu));
+            h = ft_fnv_byte(h, 0x80u | (c & 0x3Fu));
+        }
+    }
+    return h;
+}
+
+// The subword vector of tok[0..len) for columns c0 + u*32 + lane, added to s (the string's float32 sum).  The n-grams are the
+// cells (i, n) of a grid of width W = min(max_n, len + 2) - nlo + 1, walked 32 cells at a time in list order; each lane hashes
+// one cell, the kept cells' bucket ids are broadcast in order and every lane adds its columns of those rows in that order.
+__device__ __forceinline__ void ft_add_subword(const uint32_t *__restrict__ tok, int64_t len, const float *__restrict__ NG, int32_t d,
+                                               uint32_t bucket, int32_t min_n, int32_t max_n, int c0, float (&s)[FT_COLS]) {
+    const int lane = lane_id();
+    const int64_t lc = len + 2;                                        // characters of "<" + tok + ">"
+    const int64_t nlo = min_n > 1 ? min_n : 1;
+    const int64_t w = min((int64_t)max_n, lc) - nlo + 1;                 // < 2^31: max_n is an int32
+    float acc[FT_COLS];
+#pragma unroll
+    for (int u = 0; u < FT_COLS; ++u) acc[u] = 0.f;                  // gensim's word_vec = np.zeros(d, float32)
+    int64_t cnt = 0;
+    if (w > 0) {
+        const uint32_t W = (uint32_t)w;
+        // the chunk starts at cell (i0, j0); j0 < W, so j0 + 32 fits 32 bits and the divisions stay 32-bit
+        int64_t i0 = 0;
+        for (uint32_t j0 = 0; i0 < lc; i0 += (j0 + 32u) / W, j0 = (j0 + 32u) % W) {
+            const uint32_t j = j0 + (uint32_t)lane;
+            const int64_t i = i0 + j / W, n = nlo + j % W;
+            const bool keep = i + n <= lc && !(n == 1 && (i == 0 || i == lc - 1));
+            const uint32_t bid = keep ? ft_hash(tok, len, i, n) % bucket : 0u;
+            unsigned m = __ballot_sync(FULL, keep);
+            cnt += __popc(m);
+            while (m) {
+                const int q = __ffs(m) - 1;
+                m &= m - 1;
+                const float *nr = NG + (int64_t)__shfl_sync(FULL, bid, q) * d;
+#pragma unroll
+                for (int u = 0; u < FT_COLS; ++u) {
+                    const int c = c0 + u * 32 + lane;
+                    if (c < d) acc[u] = __fadd_rn(acc[u], nr[c]);
+                }
+            }
+        }
+    }
+    // word_vec / len(ngram_hashes): a float32 array over a Python int, divided in float32; no n-grams leaves the zero vector
+    const float fc = __ll2float_rn(cnt);
+#pragma unroll
+    for (int u = 0; u < FT_COLS; ++u) s[u] = __fadd_rn(s[u], cnt ? __fdiv_rn(acc[u], fc) : 0.f);
+}
+
+// One warp per string, lanes over columns: every token resolves to a float32 vector (its row of V, or its subword vector when
+// tok_row is -1), so every string pools on numpy's float32 path.  The tokens are found again by the lookup kernel's ballot walk
+// over the U+0020 breaks, in the order of tok_row.
+__global__ void __launch_bounds__(WV_THREADS) ft_pool_kernel(const uint32_t *__restrict__ blob, const int64_t *__restrict__ off, int32_t n,
+                                                            const int64_t *__restrict__ tok_off, const int32_t *__restrict__ tok_row,
+                                                            const float *__restrict__ V, const float *__restrict__ NG, int32_t d,
+                                                            uint32_t bucket, int32_t min_n, int32_t max_n, double *__restrict__ out,
+                                                            int64_t ld) {
+    const int lane = lane_id();
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += warps) {
+        const int64_t e = off[r + 1], nt = tok_off[r + 1] - tok_off[r];
+        for (int c0 = 0; c0 < d; c0 += 32 * FT_COLS) {
+            float s[FT_COLS];
+#pragma unroll
+            for (int u = 0; u < FT_COLS; ++u) s[u] = 0.f;              // numpy's add.reduce starts from +0.0
+            int64_t start = off[r], t = tok_off[r];
+            for (int64_t b0 = off[r]; b0 <= e; b0 += 32) {
+                const int64_t i = b0 + lane;
+                const bool brk = i < e ? blob[i] == 32u : i == e;
+                unsigned m = __ballot_sync(FULL, brk);
+                while (m) {                                            // the tokens ending in this chunk, in order
+                    const int64_t end = b0 + (__ffs(m) - 1);
+                    m &= m - 1;
+                    const int32_t row = tok_row[t++];
+                    if (row >= 0) {
+                        const float *vr = V + (int64_t)row * d;
+#pragma unroll
+                        for (int u = 0; u < FT_COLS; ++u) {
+                            const int c = c0 + u * 32 + lane;
+                            if (c < d) s[u] = __fadd_rn(s[u], vr[c]);
+                        }
+                    } else {
+                        ft_add_subword(blob + start, end - start, NG, d, bucket, min_n, max_n, c0, s);
+                    }
+                    start = end + 1;
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < FT_COLS; ++u) {
+                const int c = c0 + u * 32 + lane;
+                if (c < d) out[r * ld + c] = (double)__double2float_rn(__ddiv_rn((double)s[u], (double)nt));
+            }
+        }
+    }
+}
+
 static int wv_grid(int64_t warps_needed) {
     int64_t g = (warps_needed + WV_THREADS / 32 - 1) / (WV_THREADS / 32);
     if (g > SM_COUNT * 16) g = SM_COUNT * 16;
@@ -207,6 +337,19 @@ int pfz_wv_pool(const void *vectors, int32_t is_f64, int32_t d, const int64_t *t
     const int grid = wv_grid(n);
     if (is_f64) wv_pool_kernel<double><<<grid, WV_THREADS, 0, st>>>((const double *)vectors, d, tok_off, tok_row, n, out, ld);
     else wv_pool_kernel<float><<<grid, WV_THREADS, 0, st>>>((const float *)vectors, d, tok_off, tok_row, n, out, ld);
+    PFZ_LAUNCH_OK();
+    return 0;
+}
+
+int pfz_ft_pool(const uint32_t *blob, const int64_t *offsets, int32_t n, const int64_t *tok_off, const int32_t *tok_row, const float *vectors,
+                const float *vectors_ngrams, int32_t d, int64_t bucket, int32_t min_n, int32_t max_n, double *out, int64_t ld, void *stream) {
+    PFZ_REQUIRE(d >= 2 && ld >= d && n >= 0, "pfz_ft_pool: d (%d) must be >= 2 and ld (%lld) >= d", d, (long long)ld);
+    PFZ_REQUIRE(bucket >= 1 && bucket < (1ll << 32) && min_n >= 0 && max_n >= 0,
+                "pfz_ft_pool: bucket (%lld) must be in [1, 2^32) and min_n (%d), max_n (%d) >= 0", (long long)bucket, min_n, max_n);
+    if (n == 0) return 0;
+    cudaStream_t st = as_stream(stream);
+    ft_pool_kernel<<<wv_grid(n), WV_THREADS, 0, st>>>(blob, offsets, n, tok_off, tok_row, vectors, vectors_ngrams, d, (uint32_t)bucket,
+                                                       min_n, max_n, out, ld);
     PFZ_LAUNCH_OK();
     return 0;
 }
