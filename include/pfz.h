@@ -419,15 +419,16 @@ int pfz_dense_exact_fallback(const double *x_f64, const double *y_f64, int32_t n
  *
  * bound: row_thr (float[n_from]) from lists [n_lists][n_from][k_list] (global indices, -1 = empty).  exact == 0: the k-th best
  *   score of the row's union; exact != 0: with f_k the k-th best filter score and M_i the row's margin (x_norm16 / x_err16 of
- *   pfz_rows_prep_exact for these rows, y_maxima of the to-rows), tau = f_k - M_i and row_thr = tau - M_i (both rounded down)
- *   when tau > min_similarity.  -inf when no bound exists (fewer than k entries, or tau <= min_similarity).               */
+ *   pfz_rows_prep_exact for these rows, y_maxima of the to-rows), tau = f_k - M_i (-inf with fewer than k entries) and
+ *   row_thr = max(tau, min_similarity) - M_i (both rounded down).  bf16: -inf when fewer than k entries.                  */
 int pfz_dense_topn_bound(const int32_t *list_idx, const double *list_val, int32_t n_lists, int32_t n_from, int32_t k_list,
                          int32_t k, int32_t exact, const double *x_norm16, const double *x_err16, const double *y_maxima,
                          int32_t d_pad, double min_similarity, float *row_thr, void *stream);
 
-/* threshold pass: K4 (bf16, or fp16 with the filter threshold t_f of pfz_dense_cos_topk_f16) appending every (global to-index,
- * fp32 score as float64) with score >= row_thr[i] and score > min_similarity (t_f) to cand_idx / cand_val [n_from][cap] in
- * no particular order.  cand_count (int32[n_from], zeroed by the callee) counts every such to-row, also past cap: a row with
+/* threshold pass: K4 (bf16, or fp16) appending every (global to-index, fp32 score as float64) with score >= row_thr[i] to
+ * cand_idx / cand_val [n_from][cap] in no particular order; the bf16 pass also requires score > float(min_similarity), the
+ * fp16 pass ignores min_similarity (its exact row_thr already lies at or below min_similarity - M_i, and a cut at t_f would
+ * drop eligible to-rows of a row whose margin M_i exceeds M_max).  cand_count (int32[n_from], zeroed by the callee) counts every such to-row, also past cap: a row with
  * cand_count > cap must be re-run with a larger cap.  The diagonal is NOT excluded here (pfz_dense_topn_select does that).
  * The bf16 scores are the same fp32 values pfz_dense_cos_topk ranks.                                                     */
 int pfz_dense_cos_cand(const void *x_bf16, const void *y_bf16, int32_t n_from, int32_t n_to, int32_t d, double min_similarity,

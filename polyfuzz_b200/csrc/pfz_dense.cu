@@ -128,7 +128,7 @@ __device__ __forceinline__ void topk_insert(float (&tv)[KMAX], int (&ti)[KMAX], 
 
 // F16: operands are fp16 instead of bf16 (the filter pass of the exact mode); nothing else differs.
 // THRESH: the threshold epilogue of top_n > 32 (DESIGN.md 4.7) replaces the register top-k: every (j, score) with
-// score >= row_thr[i] and score > min_sim is appended to row i's candidate buffer (capacity cap; cand_cnt[i] keeps counting
+// score >= row_thr[i] and score > min_sim (-inf in the exact mode) is appended to row i's candidate buffer (capacity cap; cand_cnt[i] keeps counting
 // past it).  The four threads of a quad agree on their offsets with shuffles, so a row takes one global atomic per tile.
 // The mainloop is the same code, so the scores are the same fp32 bits as the top-k instantiations'.
 template <int KMAX, bool MCAST, bool F16, bool THRESH = false>
@@ -610,7 +610,8 @@ struct SelectParams {
 // entries are unique by index, so the ranks 0 .. n_el - 1 are distinct.  A batch of SEL_TILE entries sits in registers (SEL_PER
 // per thread) while the row streams through shared memory in tiles of SEL_TILE, so any count works; an entry stops counting
 // once its rank reaches k.  List mode writes the top k (empty slots (-1, 0.0)); bound mode writes the row threshold of the
-// threshold pass from the k-th entry (-inf when fewer than k entries are eligible, i.e. no bound: every score passes).
+// threshold pass from the k-th entry.  With fewer than k eligible entries there is no bound: the bf16 threshold is -inf (every
+// score passes), the exact one thr - M_i, which every eligible to-row passes whatever M_i is (DESIGN.md 4.7).
 __global__ void __launch_bounds__(SEL_THREADS) topn_select_kernel(const SelectParams P) {
     __shared__ double s_v[SEL_TILE];
     __shared__ int s_i[SEL_TILE];
@@ -625,7 +626,12 @@ __global__ void __launch_bounds__(SEL_THREADS) topn_select_kernel(const SelectPa
             j = P.idx[o]; v = P.val[o];
             if (j < 0 || !(v > P.thr) || (P.self_match && (long long)j == self_j)) j = -1;
         };
-        if (tid == 0) { s_nel = 0; if (P.row_thr) P.row_thr[orow] = -INFINITY; }
+        // exact bound mode: a to-row with canonical score c >= lo has filter score f >= c - M_i >= lo - M_i (rounded down)
+        auto exact_thr = [&](double lo) {
+            const double m = exact_row_margin(P.x_norm[orow], P.x_err[orow], P.y_max[0], P.y_max[1], P.gamma, P.d_pad);
+            return __double2float_rd(__dsub_rd(lo, m));
+        };
+        if (tid == 0) { s_nel = 0; if (P.row_thr) P.row_thr[orow] = P.exact ? exact_thr(P.thr_bound) : -INFINITY; }
         __syncthreads();
         for (int b0 = 0; b0 < n; b0 += SEL_TILE) {
             double ov[SEL_PER]; int oj[SEL_PER], rk[SEL_PER];
@@ -663,10 +669,10 @@ __global__ void __launch_bounds__(SEL_THREADS) topn_select_kernel(const SelectPa
                 } else if (rk[q] == P.k - 1) {
                     float rt;
                     if (!P.exact) rt = (float)ov[q];                       // an fp32 score: the threshold is the k-th score itself
-                    else {                                                 // tau = f_k - M_i; emit f >= tau - M_i when tau > thr
+                    else {                                                 // tau = f_k - M_i; emit f >= max(tau, thr) - M_i
                         const double m = exact_row_margin(P.x_norm[orow], P.x_err[orow], P.y_max[0], P.y_max[1], P.gamma, P.d_pad);
                         const double tau = __dsub_rd(ov[q], m);
-                        rt = tau > P.thr_bound ? __double2float_rd(__dsub_rd(tau, m)) : -INFINITY;
+                        rt = exact_thr(fmax(tau, P.thr_bound));
                     }
                     P.row_thr[orow] = rt;
                 }
@@ -879,8 +885,11 @@ int pfz_dense_cos_cand(const void *x_bf16, const void *y_bf16, int32_t n_from, i
 int pfz_dense_cos_cand_f16(const void *x_f16, const void *y_f16, int32_t n_from, int32_t n_to, int32_t d, double min_similarity,
                            const float *row_thr, int64_t to_index_base, int32_t n_splits, int32_t cap, int32_t *cand_idx, double *cand_val,
                            int32_t *cand_count, void *stream) {
-    return dense_cand_any<true>("pfz_dense_cos_cand_f16", x_f16, y_f16, n_from, n_to, d, filter_threshold(min_similarity, d), row_thr,
-                                to_index_base, n_splits, cap, cand_idx, cand_val, cand_count, stream);
+    // no global cut at t_f: row_thr (pfz_dense_topn_bound, exact) already holds min_similarity - M_i or more, and t_f would drop
+    // eligible to-rows of a row whose margin M_i exceeds M_max
+    (void)min_similarity;
+    return dense_cand_any<true>("pfz_dense_cos_cand_f16", x_f16, y_f16, n_from, n_to, d, -INFINITY, row_thr, to_index_base, n_splits, cap,
+                                cand_idx, cand_val, cand_count, stream);
 }
 
 static int topn_select_launch(const SelectParams &P, cudaStream_t st) {
