@@ -300,6 +300,42 @@ int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t 
                 int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
                 int32_t k, int32_t *part_idx, double *part_score, const double *gate, int32_t *counter, void *stream);
 
+/* Candidate mode of K3: each from-row scores only its own list of to-strings, e.g. TF-IDF's top-n for that row.
+ * Replaces: the blocking step users run around the reference -- TF-IDF's top-n per from-string, then rapidfuzz's
+ *           process.extractOne / process.extract(query, [to_list[j] for j in candidates], scorer, ...) (the scorer loop of
+ *           polyfuzz/models/_rapidfuzz.py:99-113 and polyfuzz/models/_distance.py:89-102 restricted to those pairs).
+ * Same parameters, metrics, cutoffs, self-exclusion, key and kernels as the all-pairs sibling, without n_splits, plus
+ *   cand_idx: int32[n_from][c] to-indices per from-row, distinct within a row, -1 = empty slot (TF-IDF's top_idx)
+ *   pos_of:   int32[n_to] the sorted position of each to-index (the inverse of pfz_lev_pack's `order`)
+ * Outputs: one list per row, no merge -- best_* int32 / float64 / int32 [n_from] (argbest; (-1, 0.0, -1) for a row with no
+ * candidate that passes), top_* [n_from][k] (topk; empty slots (-1, 0.0)).  A row's result is that of the all-pairs entry
+ * point against the to-strings of its list, bit for bit.  matrix (argbest, may be NULL): only the candidate pairs' cells are
+ * written.  gate (DL, may be NULL): a lower bound of the row's k-th best score over its candidates.  counter: int32[1]. */
+int pfz_lev_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                         int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
+                         const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
+                         int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                         const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
+                         int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, int32_t *counter, void *stream);
+int pfz_lev_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                      int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
+                      const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
+                      int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                      const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
+                      int32_t *counter, void *stream);
+int pfz_dl_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                        int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
+                        const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
+                        int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                        const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
+                        int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream);
+int pfz_dl_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
+                     int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
+                     const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
+                     int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                     const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
+                     const double *gate, int32_t *counter, void *stream);
+
 /* K3b  rapidfuzz's token / partial / weighted scorers with a fused per-row arg-best (csrc/pfz_fuzz.cu).
  * Replaces: process.extractOne(query, to_list, scorer=fuzz.WRatio | partial_ratio | token_*_ratio | ..., score_cutoff) at
  *           polyfuzz/models/_rapidfuzz.py:48,106-108 and the scorer loop of polyfuzz/models/_distance.py:98.
@@ -354,6 +390,18 @@ int pfz_tok_remap(const int32_t *tok_ptr, const int32_t *ids_in, int32_t n, cons
 int pfz_fuzz_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
                   int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k,
                   void *stream);
+
+/* Candidate mode of K3b (see pfz_lev_cand_argbest): the siblings' scorers, cutoffs and key over each from-row's own list.
+ * Replaces: process.extractOne / process.extract(query, [to_list[j] for j in candidates], scorer=fuzz.WRatio | ..., ...) --
+ *           the reference's RapidFuzz scorer loop (polyfuzz/models/_rapidfuzz.py:106-108) over a blocked candidate set.
+ * ptrs: as pfz_fuzz_argbest, except part_idx / part_score are the outputs: [n_from] (argbest) or [n_from][k] (topk);
+ * cand_idx int32[n_from][c] and pos_of int32[n_to] as in pfz_lev_cand_argbest; counter int32[1].                            */
+int pfz_fuzz_cand_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
+                          int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
+                          int32_t c, const int32_t *pos_of, void *stream);
+int pfz_fuzz_cand_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
+                       int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
+                       int32_t c, const int32_t *pos_of, int32_t k, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K4  dense cosine top-k for pre-computed embeddings (bf16 wgmma GEMM fed by TMA, top-k fused into the

@@ -124,6 +124,48 @@ __device__ __forceinline__ GroupRange split_groups(int n_to, int n_splits) {
     return {lo, min(n_grp, lo + per)};
 }
 
+// ---- the row driver's to-source: every to-string (CAND = false) or a candidate list per from-row (CAND = true) -----------
+// A row is walked in steps [lo, hi) of 32 to-strings, one per lane.  All-pairs: step g is to-group g of the block's split and
+// lane l takes sorted position 32g + l.  Candidate mode: step t is candidates 32t .. 32t + 31 of the row's list and lane l
+// takes cand[i][32t + l] (-1: nothing to score), found at sorted position pos_of[j] (the inverse of the layout's `order`),
+// i.e. group p / 32, lane p % 32 of the same packed layout.  One list per row, so candidate mode has one split.
+struct CandList {
+    const int32_t *idx;                 // int32 [n_from][c] to-indices (distinct per row), -1 = empty slot
+    int c;                              // list length per row
+    const int32_t *pos_of;              // int32 [n_to] sorted position of each to-index
+};
+
+template <bool CAND>
+__device__ __forceinline__ GroupRange to_steps(int n_to, int n_splits, const CandList &cl) {
+    if constexpr (CAND) return {0, (cl.c + 31) >> 5};
+    else return split_groups(n_to, n_splits);
+}
+
+// the sorted position p the lane scores at step s of row i; to_have(p) tells whether there is one (all-pairs: p < n_to,
+// candidate mode: p >= 0)
+template <bool CAND>
+__device__ __forceinline__ int to_pos(int s, int i, const CandList &cl) {
+    if constexpr (CAND) {
+        const int q = s * 32 + lane_id();
+        const int j = q < cl.c ? cl.idx[(size_t)i * cl.c + q] : -1;
+        return j >= 0 ? cl.pos_of[j] : -1;
+    } else {
+        return s * 32 + lane_id();
+    }
+}
+template <bool CAND>
+__device__ __forceinline__ bool to_have(int p, int n_to) { return CAND ? p >= 0 : p < n_to; }
+
+// The lane's packed column (lane-strided words) in the layout (packed, grp_word_off) at step s for sorted position p.  A lane
+// with nothing to score in candidate mode gets the layout's first column and length 0.  The warp-uniform text loops read up
+// to the warp's longest string in every lane; that stays inside `packed` in candidate mode too, because groups are in
+// ascending length order, so no group ends closer to the buffer's end than the longest string's words.
+template <bool CAND>
+__device__ __forceinline__ const uint32_t *to_column(const uint32_t *packed, const int64_t *grp_word_off, int s, int p) {
+    if constexpr (CAND) return p >= 0 ? packed + grp_word_off[p >> 5] + (p & 31) : packed + lane_id();
+    else return packed + grp_word_off[s] + lane_id();
+}
+
 // the warp's next from-row (from_ids[q], q from the split's counter), or -1 once all n_ids rows are taken
 __device__ __forceinline__ int claim_row(int32_t *counter, const int32_t *from_ids, int n_ids) {
     int q = 0;

@@ -51,6 +51,7 @@ struct FuzzParams {
     int scorer; double cutoff; int exclude_self; int64_t self_shift;
     int n_splits; int32_t *part_idx; double *part_score; int n_from; int32_t *counter;
     int k;                                                  // top-k epilogue: list length; part_* are [n_splits][n_from][k]
+    CandList cand;                                          // candidate mode: the rows' to-lists (n_splits = 1)
 };
 
 // ---- scalar scorer algebra (double, no contraction) -- mirrors oracle/fuzz.py line by line -------------------------------------
@@ -252,6 +253,8 @@ __device__ int fz_diff_indel(const uint64_t *__restrict__ peq_u, const int32_t *
 
 // TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings
 // (the group's body is a do/while(0), so a lane that skips its pair still reaches the warp-wide offer).
+// CAND = true: the row's candidate list instead of the split's to-groups (to_steps / to_pos / to_column of pfz_common.cuh);
+// CTA rows take its steps of 32 in turn, as they take to-groups.
 // (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; for the arg-best
 // classes at 1 and 2 words, the blocks per SM their shared memory and registers allow, which keeps ptxas from spilling more)
 // CTA_ROW (NW >= 8): dyn holds the masks of the variants the scorer reads (fz_variants), in variant order, then the merge
@@ -262,7 +265,7 @@ __host__ __device__ constexpr bool fz_reads_uniq(int sc) { return sc == FZ_TSET 
 __host__ __device__ constexpr int fz_variants(int sc) { return (int)fz_reads_plain(sc) + (int)fz_reads_sorted(sc) + (int)fz_reads_uniq(sc); }
 constexpr size_t fz_cta_smem(int nw, int warps, int sc) { return (size_t)fz_variants(sc) * 256 * nw * 8 + (size_t)warps * 32 * 12 + 16; }
 
-template <int NW, int WARPS, bool TOPK = false>
+template <int NW, int WARPS, bool TOPK = false, bool CAND = false>
 __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : NW == 1 ? 6 : NW == 2 ? 9 : 0) fuzz_kernel(const FuzzParams P) {
     constexpr bool CTA_ROW = NW >= 8;
     extern __shared__ __align__(16) unsigned char dyn[];
@@ -289,7 +292,7 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : NW == 1 ? 6 : NW == 2 ?
         if constexpr (CTA_ROW) i = claim_row_cta(P.counter + blockIdx.y, P.from_ids, P.n_ids, slot);
         else i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
         if (i < 0) break;
-        const GroupRange gr = split_groups(P.n_to, P.n_splits);    // per row: held across rows, it adds spills (2 words)
+        const GroupRange gr = to_steps<CAND>(P.n_to, P.n_splits, P.cand);    // per row: held across rows, it adds spills (2 words)
         int lens[3];
         for (int v = 0; v < 3; ++v) {
             const int64_t fb = P.F.off[v][i];
@@ -317,13 +320,13 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : NW == 1 ? 6 : NW == 2 ?
         for (int g = gr.lo + (CTA_ROW ? w : 0); g < gr.hi; g += CTA_ROW ? WARPS : 1) {
             double cand_s = 0.0; int cand_j = -1;
             do {
-                const int p = g * 32 + lane;
-                if (p >= P.n_to) continue;
+                const int p = to_pos<CAND>(g, i, P.cand);
+                if (!to_have<CAND>(p, P.n_to)) continue;
                 const int orig = P.sorig[p];
                 if (P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) continue;
-                TextRef t0{P.packed[0] + P.grp_off[0][g] + lane, P.slen[0][p]};
-                TextRef t1{P.packed[1] + P.grp_off[1][g] + lane, P.slen[1][p]};
-                TextRef t2{P.packed[2] + P.grp_off[2][g] + lane, P.slen[2][p]};
+                TextRef t0{to_column<CAND>(P.packed[0], P.grp_off[0], g, p), P.slen[0][p]};
+                TextRef t1{to_column<CAND>(P.packed[1], P.grp_off[1], g, p), P.slen[1][p]};
+                TextRef t2{to_column<CAND>(P.packed[2], P.grp_off[2], g, p), P.slen[2][p]};
                 const int lb = t0.n;
                 const double cut = P.cutoff;
                 // token-set facts of the pair, computed on demand
@@ -431,21 +434,23 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : NW == 1 ? 6 : NW == 2 ?
     }
 }
 
-template <int NW, bool TOPK>
+template <int NW, bool TOPK, bool CAND>
 static int launch_fuzz(const FuzzParams &P, int sms, cudaStream_t st) {
     if constexpr (NW >= 8) {
         constexpr int WARPS = 4;
-        return launch_ctas(fuzz_kernel<NW, WARPS, TOPK>, WARPS, fz_cta_smem(NW, WARPS, P.scorer), P.n_ids, P.n_splits, sms, st, P);
+        return launch_ctas(fuzz_kernel<NW, WARPS, TOPK, CAND>, WARPS, fz_cta_smem(NW, WARPS, P.scorer), P.n_ids, P.n_splits, sms, st, P);
     } else {
         constexpr int WARPS = NW == 1 ? 4 : NW == 2 ? 2 : 1;
-        return launch_rows(fuzz_kernel<NW, WARPS, TOPK>, WARPS, (size_t)WARPS * 3 * 256 * NW * 8, P.n_ids, P.n_splits, sms, st, P);
+        return launch_rows(fuzz_kernel<NW, WARPS, TOPK, CAND>, WARPS, (size_t)WARPS * 3 * 256 * NW * 8, P.n_ids, P.n_splits, sms, st, P);
     }
 }
 
-// the 38 pointers of the C ABI (order: include/pfz.h) -> FuzzParams; part_idx / part_score as the caller's entry point lays them out
-template <bool TOPK>
+// the 38 pointers of the C ABI (order: include/pfz.h) -> FuzzParams; part_idx / part_score as the caller's entry point lays them out.
+// CAND: the candidate entry points (cl: the rows' lists, n_splits = 1).
+template <bool TOPK, bool CAND = false>
 static int run_fuzz(const void *const *ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
-                    double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k_out, void *stream) {
+                    double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k_out, void *stream,
+                    const CandList &cl = CandList{nullptr, 0, nullptr}) {
     cudaStream_t st = as_stream(stream);
     FuzzParams P;
     int k = 0;
@@ -461,14 +466,14 @@ static int run_fuzz(const void *const *ptrs, int32_t n_from, int32_t n_ids, int3
     P.part_idx = (int32_t *)ptrs[k++]; P.part_score = (double *)ptrs[k++]; P.counter = (int32_t *)ptrs[k++];                  // 37
     k++;                                                                            // 38: reserved
     P.n_ids = n_ids; P.n_to = n_to; P.scorer = scorer; P.cutoff = score_cutoff; P.exclude_self = exclude_self; P.self_shift = self_shift;
-    P.n_splits = n_splits; P.n_from = n_from; P.k = k_out;
+    P.n_splits = n_splits; P.n_from = n_from; P.k = k_out; P.cand = cl;
     int sms = 0;
     if (start_rows(P.counter, n_splits, st, &sms)) return 1;
-    if (n_words == 1) return launch_fuzz<1, TOPK>(P, sms, st);
-    if (n_words == 2) return launch_fuzz<2, TOPK>(P, sms, st);
-    if (n_words == 4) return launch_fuzz<4, TOPK>(P, sms, st);
-    if (n_words == 8) return launch_fuzz<8, TOPK>(P, sms, st);
-    return launch_fuzz<16, TOPK>(P, sms, st);
+    if (n_words == 1) return launch_fuzz<1, TOPK, CAND>(P, sms, st);
+    if (n_words == 2) return launch_fuzz<2, TOPK, CAND>(P, sms, st);
+    if (n_words == 4) return launch_fuzz<4, TOPK, CAND>(P, sms, st);
+    if (n_words == 8) return launch_fuzz<8, TOPK, CAND>(P, sms, st);
+    return launch_fuzz<16, TOPK, CAND>(P, sms, st);
 }
 
 }  // namespace pfz
@@ -500,5 +505,36 @@ int pfz_fuzz_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32
     PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_fuzz_topk: k=%d unsupported (1..32)", k);
     if (n_ids <= 0 || n_to <= 0) return 0;
     return run_fuzz<true>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, n_splits, k, stream);
+}
+
+/* ptrs: as pfz_fuzz_argbest, with part_idx / part_score the outputs best_idx int32[n_from] / best_score float64[n_from] */
+int pfz_fuzz_cand_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
+                          int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
+                          int32_t c, const int32_t *pos_of, void *stream) {
+    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_cand_argbest: expected 38 pointers, got %d", n_ptrs);
+    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_cand_argbest: unknown scorer %d", scorer);
+    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_fuzz_cand_argbest: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
+    PFZ_REQUIRE(c >= 0 && (c == 0 || (cand_idx && pos_of)), "pfz_fuzz_cand_argbest: c=%d with cand_idx %p, pos_of %p", c,
+                (const void *)cand_idx, (const void *)pos_of);
+    if (n_ids <= 0 || n_to <= 0) return 0;
+    return run_fuzz<false, true>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, 1, 1, stream,
+                                 CandList{cand_idx, c, pos_of});
+}
+
+/* ptrs: as pfz_fuzz_argbest, with part_idx / part_score the outputs top_idx int32[n_from][k] / top_score float64[n_from][k] */
+int pfz_fuzz_cand_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
+                       int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
+                       int32_t c, const int32_t *pos_of, int32_t k, void *stream) {
+    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_cand_topk: expected 38 pointers, got %d", n_ptrs);
+    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_cand_topk: unknown scorer %d", scorer);
+    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_fuzz_cand_topk: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
+    PFZ_REQUIRE(c >= 0 && (c == 0 || (cand_idx && pos_of)), "pfz_fuzz_cand_topk: c=%d with cand_idx %p, pos_of %p", c,
+                (const void *)cand_idx, (const void *)pos_of);
+    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_fuzz_cand_topk: k=%d unsupported (1..32)", k);
+    if (n_ids <= 0 || n_to <= 0) return 0;
+    return run_fuzz<true, true>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, 1, k, stream,
+                                CandList{cand_idx, c, pos_of});
 }
 }

@@ -65,11 +65,12 @@ struct LevParams {
     const uint32_t *packed; const int64_t *grp_word_off; const int32_t *slen; const int32_t *sorig; int n_to;
     int metric; double cutoff; int exclude_self; int64_t self_shift;
     double ratio_min_ns;                // RATIO: its cutoff as one test ns >= ratio_min_ns (ratio_min_ns_of)
-    int n_splits;                       // to-groups are split over blockIdx.y
+    int n_splits;                       // to-groups are split over blockIdx.y (candidate mode: 1)
     int32_t *part_idx; double *part_score; int32_t *part_dist;     // [n_splits][n_from]
     int32_t *matrix; int64_t matrix_ld;                           // optional full matrix [n_from][n_to]
     int n_from; int32_t *counter;
     int k;                              // top-k epilogue: list length; part_idx / part_score are [n_splits][n_from][k]
+    CandList cand;                      // candidate mode: the rows' to-lists (to_steps / to_pos / to_column)
 };
 
 __device__ __forceinline__ double ratio_ns(int d, int la, int lb) {      // Indel.normalized_similarity
@@ -195,8 +196,9 @@ struct LevColumn {
 // One warp scores pattern `pat` against every to-string of its split.  LCS = false: Levenshtein, or with OSA = true optimal
 // string alignment (LevColumn); LCS = true: longest common subsequence (Hyyro 2004) -> Indel = la + lb - 2*LCS.
 // TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings.
+// CAND = true: the row's candidate list instead of the split's to-groups (to_steps / to_pos / to_column of pfz_common.cuh).
 // (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; 0 = unspecified)
-template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false, bool OSA = false>
+template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false, bool OSA = false, bool CAND = false>
 __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const LevParams P) {
     static_assert(!(OSA && LCS), "OSA extends the Levenshtein recurrence");
     constexpr int B = WordOps<W>::BITS;
@@ -208,7 +210,7 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
     for (;;) {
         const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
         if (i < 0) break;
-        const GroupRange gr = split_groups(P.n_to, P.n_splits);    // per row: held across rows, ptxas spilled it (LCS, 8+ words)
+        const GroupRange gr = to_steps<CAND>(P.n_to, P.n_splits, P.cand);    // per row: held across rows, ptxas spilled it (LCS, 8+ words)
         const int64_t fb = P.from_off[i];
         const int m = (int)(P.from_off[i + 1] - fb);
         build_peq<W, NW>(peq, P.from_blob + fb, m, P.sym_table);
@@ -220,11 +222,11 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
         if constexpr (TOPK) top.init(P.k); else best.init();
         for (int g = gr.lo; g < gr.hi; ++g) {
             double cand_s = 0.0; int cand_j = -1;
-            const int p = g * 32 + lane;
-            const bool have = p < P.n_to;
+            const int p = to_pos<CAND>(g, i, P.cand);
+            const bool have = to_have<CAND>(p, P.n_to);
             const int n = have ? P.slen[p] : 0;
             const int orig = have ? P.sorig[p] : -1;
-            const uint32_t *src = P.packed + P.grp_word_off[g] + lane;
+            const uint32_t *src = to_column<CAND>(P.packed, P.grp_word_off, g, p);
             int dist;
             if constexpr (!LCS) {
                 LevColumn<W, NW, OSA> col;
@@ -305,7 +307,7 @@ template <typename W> __device__ __forceinline__ int low_bit(W x);
 template <> __device__ __forceinline__ int low_bit<uint32_t>(uint32_t x) { return __ffs(x) - 1; }
 template <> __device__ __forceinline__ int low_bit<uint64_t>(uint64_t x) { return __ffsll(x) - 1; }
 
-template <typename W, int NW, int WARPS, bool TOPK = false>
+template <typename W, int NW, int WARPS, bool TOPK = false, bool CAND = false>
 __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
     constexpr int B = WordOps<W>::BITS;
     constexpr int STORE = B * NW;                                           // max matches per lane
@@ -315,7 +317,7 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
     W *peq = reinterpret_cast<W *>(dyn) + (size_t)w * 256 * NW;              // peq[sym * NW + block]
     uint8_t *store = dyn + (size_t)WARPS * 256 * NW * sizeof(W) + (size_t)w * STORE * 32 + lane;    // store[k * 32]
     const bool winkler = P.metric == PFZ_METRIC_JARO_WINKLER;
-    const GroupRange gr = split_groups(P.n_to, P.n_splits);
+    const GroupRange gr = to_steps<CAND>(P.n_to, P.n_splits, P.cand);
 
     for (;;) {
         const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
@@ -330,8 +332,8 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
         if constexpr (TOPK) top.init(P.k); else best.init();
         for (int g = gr.lo; g < gr.hi; ++g) {
             double cand_s = 0.0; int cand_j = -1;
-            const int p = g * 32 + lane;
-            const bool have = p < P.n_to;
+            const int p = to_pos<CAND>(g, i, P.cand);
+            const bool have = to_have<CAND>(p, P.n_to);
             const int n = have ? P.slen[p] : 0;
             const int orig = have ? P.sorig[p] : -1;
             const int R = max(0, max(m, n) / 2 - 1);
@@ -339,7 +341,7 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
             int jmax = jend;
 #pragma unroll
             for (int d = 16; d; d >>= 1) jmax = max(jmax, __shfl_xor_sync(FULL, jmax, d));
-            const uint32_t *src = P.packed + P.grp_word_off[g] + lane;
+            const uint32_t *src = to_column<CAND>(P.packed, P.grp_word_off, g, p);
             const uint32_t first = n > 0 ? src[0] : 0u;
             W F[NW], win[NW];                                                // win: pattern bits j-R .. j+R
 #pragma unroll
@@ -484,7 +486,7 @@ __device__ __forceinline__ int dl_dp(const uint8_t *__restrict__ pat, int m, con
     return last;
 }
 
-template <typename W, int NW, int WARPS, bool TOPK>
+template <typename W, int NW, int WARPS, bool TOPK, bool CAND = false>
 __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, const double *__restrict__ gate) {
     constexpr int B = WordOps<W>::BITS;
     using Lay = DlLayout<W, NW>;
@@ -500,7 +502,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, co
     const bool norm = P.metric == PFZ_METRIC_NORM_DL;
     const bool full = P.matrix != nullptr;                                  // matrix mode: the DP on every pair
     const double NEG_INF = -CUDART_INF;
-    const GroupRange gr = split_groups(P.n_to, P.n_splits);
+    const GroupRange gr = to_steps<CAND>(P.n_to, P.n_splits, P.cand);
 
     for (;;) {
         const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
@@ -553,11 +555,11 @@ __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, co
         };
 
         for (int g = gr.lo; g < gr.hi; ++g) {
-            const int p = g * 32 + lane;
-            const bool have = p < P.n_to;
+            const int p = to_pos<CAND>(g, i, P.cand);
+            const bool have = to_have<CAND>(p, P.n_to);
             const int n = have ? P.slen[p] : 0;
             const int orig = have ? P.sorig[p] : -1;
-            const uint32_t *src = P.packed + P.grp_word_off[g] + lane;
+            const uint32_t *src = to_column<CAND>(P.packed, P.grp_word_off, g, p);
             LevColumn<W, NW, true> col;
             col.init();
             int score_m = m;
@@ -613,7 +615,7 @@ static int dispatch_words(int n_words, F &&f) {
 }
 
 // word class -> kernel instantiation; the metric picks Levenshtein, Indel, OSA, Jaro or DL (gate: DL only)
-template <bool TOPK>
+template <bool TOPK, bool CAND>
 static int launch_class(const LevParams &P, const double *gate, int n_words, int sms, cudaStream_t st) {
     const int mt = P.metric;
     return dispatch_words(n_words, [&](auto c) {
@@ -624,45 +626,48 @@ static int launch_class(const LevParams &P, const double *gate, int n_words, int
             // to 256 symbols, 2 at 512, 1 at 1 024.
             constexpr size_t PER_WARP = DlLayout<W, NW>::PER_WARP;
             constexpr int WARPS = warps_within(PER_WARP, 227 * 1024);
-            return launch_rows(dl_kernel<W, NW, WARPS, TOPK>, WARPS, WARPS * PER_WARP, P.n_ids, P.n_splits, sms, st, P, gate);
+            return launch_rows(dl_kernel<W, NW, WARPS, TOPK, CAND>, WARPS, WARPS * PER_WARP, P.n_ids, P.n_splits, sms, st, P, gate);
         }
         if (mt == PFZ_METRIC_JARO || mt == PFZ_METRIC_JARO_WINKLER) {
             // Shared memory per warp: Peq (256 x NW words) plus the match store (32 lanes x B*NW bytes), the same size again.
             // Up to 64 KB per CTA: 4 warps up to 256 code points, 2 at 512, 1 at 1 024.
             constexpr size_t PER_WARP = 2 * 256 * NW * sizeof(W);
             constexpr int WARPS = warps_within(PER_WARP, 65536);
-            return launch_rows(jaro_kernel<W, NW, WARPS, TOPK>, WARPS, WARPS * PER_WARP, P.n_ids, P.n_splits, sms, st, P);
+            return launch_rows(jaro_kernel<W, NW, WARPS, TOPK, CAND>, WARPS, WARPS * PER_WARP, P.n_ids, P.n_splits, sms, st, P);
         }
         constexpr int WARPS = 4;
         const size_t smem = (size_t)WARPS * 256 * NW * sizeof(W);
         if (mt == PFZ_METRIC_OSA || mt == PFZ_METRIC_NORM_OSA)
-            return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK, true>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+            return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK, true, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
         if (mt == PFZ_METRIC_INDEL || mt == PFZ_METRIC_RATIO)
-            return launch_rows(lev_kernel<W, NW, true, WARPS, TOPK>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
-        return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+            return launch_rows(lev_kernel<W, NW, true, WARPS, TOPK, false, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+        return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK, false, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
     });
 }
 
-// The body of the four K3 entry points after their metric checks: the checks they share, the row counters and the launch.
-// fn names the entry point in error messages.
-template <bool TOPK>
+// The body of the K3 entry points after their metric checks: the checks they share, the row counters and the launch.
+// fn names the entry point in error messages.  CAND: the candidate entry points (cl: the rows' lists, n_splits = 1).
+template <bool TOPK, bool CAND = false>
 static int run_k3(const char *fn, const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
                   int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off,
                   const int32_t *slen, const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self,
                   int64_t self_shift, int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, int32_t *part_dist,
-                  int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream) {
+                  int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream,
+                  const CandList &cl = CandList{nullptr, 0, nullptr}) {
     PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
                 "%s: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", fn, n_words);
     PFZ_REQUIRE(n_splits >= 1, "%s: n_splits < 1", fn);
     PFZ_REQUIRE(!TOPK || (k >= 1 && k <= 32), "%s: k=%d unsupported (1..32)", fn, k);
+    PFZ_REQUIRE(!CAND || (cl.c >= 0 && (cl.c == 0 || (cl.idx && cl.pos_of))), "%s: c=%d with cand_idx %p, pos_of %p", fn, cl.c,
+                (const void *)cl.idx, (const void *)cl.pos_of);
     if (n_ids <= 0 || n_to < 0) return 0;
     cudaStream_t st = as_stream(stream);
     int sms = 0;
     if (start_rows(counter, n_splits, st, &sms)) return 1;
     LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
                 exclude_self, self_shift, ratio_min_ns_of(score_cutoff), n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from,
-                counter, k};
-    return launch_class<TOPK>(P, gate, n_words, sms, st);
+                counter, k, cl};
+    return launch_class<TOPK, CAND>(P, gate, n_words, sms, st);
 }
 
 }  // namespace pfz
@@ -725,6 +730,54 @@ int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t 
     return run_k3<true>("pfz_dl_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
                         slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, k, part_idx, part_score, nullptr,
                         nullptr, 0, gate, counter, stream);
+}
+
+int pfz_lev_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                         int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                         const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                         const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
+                         int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_OSA, "pfz_lev_cand_argbest: unknown metric %d", metric);
+    const bool jaro = metric == PFZ_METRIC_JARO || metric == PFZ_METRIC_JARO_WINKLER;
+    PFZ_REQUIRE(!(jaro && matrix), "pfz_lev_cand_argbest: the distance matrix is not available for the Jaro metrics (matrix must be NULL)");
+    return run_k3<false, true>("pfz_lev_cand_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
+                               grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, 1, best_idx, best_score,
+                               best_dist, matrix, matrix_ld, nullptr, counter, stream, CandList{cand_idx, c, pos_of});
+}
+
+int pfz_lev_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                      int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                      const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                      const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
+                      int32_t *counter, void *stream) {
+    PFZ_REQUIRE((metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER) || metric == PFZ_METRIC_NORM_OSA,
+                "pfz_lev_cand_topk: metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA)", metric);
+    return run_k3<true, true>("pfz_lev_cand_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
+                              grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, k, top_idx, top_score,
+                              nullptr, nullptr, 0, nullptr, counter, stream, CandList{cand_idx, c, pos_of});
+}
+
+int pfz_dl_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                        int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                        const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                        const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
+                        int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(metric == PFZ_METRIC_DL || metric == PFZ_METRIC_NORM_DL, "pfz_dl_cand_argbest: metric %d unsupported (DL, NORM_DL)", metric);
+    PFZ_REQUIRE(!(matrix && gate), "pfz_dl_cand_argbest: the distance matrix needs every pair, so gate must be NULL with a matrix");
+    return run_k3<false, true>("pfz_dl_cand_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
+                               grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, 1, best_idx, best_score,
+                               best_dist, matrix, matrix_ld, gate, counter, stream, CandList{cand_idx, c, pos_of});
+}
+
+int pfz_dl_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                     int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                     const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
+                     const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
+                     const double *gate, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(metric == PFZ_METRIC_NORM_DL, "pfz_dl_cand_topk: metric %d unsupported (NORM_DL)", metric);
+    return run_k3<true, true>("pfz_dl_cand_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
+                              grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, k, top_idx, top_score,
+                              nullptr, nullptr, 0, gate, counter, stream, CandList{cand_idx, c, pos_of});
 }
 
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits, int32_t n_from,

@@ -23,6 +23,10 @@ Two levels: `EditQueries` / `EditTargets` stage a from-list / to-list in HBM onc
 alphabet batches); `edit_argbest_staged` only enqueues kernels, so a staged pair can be scored repeatedly
 (bench.py's device-timed leg, the multi-GPU shards) without touching the host lists again.  `KeptTargets` holds a
 matcher's last staged to-side, which a `re_train=False` call with an equal to-list scores against again.
+
+Candidate mode (`edit_cand_topk_staged`, DESIGN.md 4.16): each from-row scores only the to-indices of its row of a device
+int32 [n_from, c] candidate array (-1 = empty slot, distinct per row; TF-IDF's top-n), with the same kernels, scores, cutoffs
+and key, so a row equals the all-pairs result against the to-strings of its list.
 """
 import numpy as np
 import torch
@@ -87,6 +91,13 @@ def group_word_offsets(lens):
     return goff
 
 
+def inverse_order(order):
+    """pos_of[order[p]] = p: the sorted position of every to-index (the candidate kernels' pos_of)."""
+    pos_of = np.empty(len(order), dtype=np.int32)
+    pos_of[order] = np.arange(len(order), dtype=np.int32)
+    return pos_of
+
+
 def _blob_to_dev(b):
     if b.size == 0:
         return torch.zeros(1, dtype=torch.int32, device=_dev())
@@ -146,7 +157,8 @@ class EditTargets:
         self.n_grp = (self.n + 31) // 32
         goff = group_word_offsets(tlens[order])
         self.d_order = _to_dev(order); self.d_goff = _to_dev(goff)
-        self.h2d_bytes += order.nbytes + goff.nbytes
+        self.d_pos_of = _to_dev(inverse_order(order))        # candidate mode: to-index -> sorted position
+        self.h2d_bytes += order.nbytes + goff.nbytes + order.nbytes
         self.packed = torch.empty(max(int(goff[-1]), 1), dtype=torch.int32, device=dev)
         self.slen = torch.empty(self.n, dtype=torch.int32, device=dev)
 
@@ -327,3 +339,63 @@ def lev_merge(part_idx, part_score, part_dist):
     _lib.call("pfz_lev_merge", _p(part_idx.contiguous()), _p(part_score.contiguous()), _p(part_dist.contiguous()), n_lists, n_from,
               _p(bi), _p(bs), _p(bd), _stream())
     return bi[:n_from], bs[:n_from], bd[:n_from]
+
+
+def check_candidates(cand, n_from, n_to):
+    """A candidate array for the cand kernels: a CUDA int32 tensor [n_from, c] (made contiguous) whose entries are to-indices
+    in [0, n_to) or -1.  Indices must be distinct within a row (the top-k epilogue needs it; TF-IDF's rows are); that is not
+    checked.  The range check costs one device-to-host read."""
+    import torch as _t
+    if not isinstance(cand, _t.Tensor) or cand.dtype != _t.int32 or cand.dim() != 2 or not cand.is_cuda:
+        raise ValueError("candidates must be a CUDA int32 tensor [n_from, c]")
+    if cand.shape[0] != n_from:
+        raise ValueError(f"candidates have {cand.shape[0]} rows for {n_from} from-strings")
+    cand = cand.contiguous()
+    if cand.numel() and bool(((cand < -1) | (cand >= n_to)).any()):
+        raise ValueError(f"candidate indices must lie in [-1, {n_to})")
+    return cand
+
+
+def edit_cand_topk_staged(Q, T, cand, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0):
+    """Kernels only (pfz_lev_cand_* / pfz_dl_cand_*): per from-row the k best to-strings among its candidates cand[i]
+    (check_candidates), under the metrics, cutoffs, self-exclusion and key of edit_argbest_staged / edit_topk_staged.
+    k = 1 returns what edit_argbest_staged returns (best_idx, best_score, best_dist), any metric; k > 1 returns
+    (idx int32[n_from, k], score float64[n_from, k]) as edit_topk_staged, metrics TOPK_METRICS.  A row with no candidate that
+    passes gets (-1, 0.0).  dl / norm_dl run without the OSA gate (a row's list is short)."""
+    k = check_top_n(k)
+    if k > 1 and metric not in TOPK_METRICS:
+        raise ValueError(f"top-k is available for the metrics {TOPK_METRICS}, not {metric!r}")
+    if metric not in METRIC:
+        raise ValueError(f"unknown metric {metric!r}")
+    dev = _dev()
+    n_from, n_to = Q.n, T.n
+    cand = check_candidates(cand, n_from, n_to)
+    c = int(cand.shape[1])
+    shape = (max(n_from, 1),) if k == 1 else (max(n_from, 1), k)
+    idx = torch.full(shape, -1, dtype=torch.int32, device=dev)
+    score = torch.zeros(shape, dtype=torch.float64, device=dev)
+    dist = torch.full(shape, -1, dtype=torch.int32, device=dev) if k == 1 else None
+    if n_from and n_to and c:
+        counter = torch.zeros(1, dtype=torch.int32, device=dev)
+        dl = metric in DL_GATE
+        for cls in _word_classes(Q, T):
+            head = _k3_head(Q, T, cls, metric, score_cutoff, exclude_self, self_shift, 1)[:-1] + (_p(cand), c, _p(T.d_pos_of))
+            gate = (None,) if dl else ()
+            if k == 1:
+                _lib.call("pfz_dl_cand_argbest" if dl else "pfz_lev_cand_argbest", *head, _p(idx), _p(score), _p(dist), None, 0, *gate,
+                          _p(counter), _stream())
+            else:
+                _lib.call("pfz_dl_cand_topk" if dl else "pfz_lev_cand_topk", *head, k, _p(idx), _p(score), *gate, _p(counter),
+                          _stream())
+    if k == 1:
+        return idx[:n_from], score[:n_from], dist[:n_from]
+    return idx[:n_from], score[:n_from]
+
+
+def edit_cand_topk(from_list, to_list, cand, k, metric="ratio", score_cutoff=0.0, exclude_self=False, kept=None, reuse=False):
+    """Host lists in, device tensors out (see edit_cand_topk_staged); kept and reuse as in edit_argbest."""
+    k = check_top_n(k)
+    _dev()
+    Q = EditQueries(from_list)
+    T = kept.stage(("k3", 0), to_list, EditTargets, reuse) if kept is not None else EditTargets(to_list)
+    return edit_cand_topk_staged(Q, T, cand, k, metric, score_cutoff, exclude_self)

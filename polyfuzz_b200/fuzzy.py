@@ -12,6 +12,8 @@ signature of the ids; every score is computed on the device.
 A to-list is staged once into a `FuzzTargets` (its token tables, length order and pack buffers), which depends on no
 from-list: a matcher keeps it across calls (editdist.KeptTargets), and each call only tokenises the from-list, joins the two
 vocabularies and renumbers the kept to-side ids to the union (pfz_tok_union, pfz_tok_remap).
+
+`fuzz_cand_topk` scores each from-row against its own candidate list only (editdist.check_candidates; DESIGN.md 4.16).
 """
 import ctypes
 
@@ -19,7 +21,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .editdist import _alphabet_batches, _blob_to_dev, check_top_n, default_splits, group_word_offsets, symbol_table
+from .editdist import (_alphabet_batches, _blob_to_dev, check_candidates, check_top_n, default_splits, group_word_offsets,
+                       inverse_order, symbol_table)
 from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
@@ -84,6 +87,7 @@ class FuzzTargets:
         order = np.argsort(lens[0], kind="stable").astype(np.int32)
         self.n_grp = (self.n + 31) // 32
         self.d_order = _to_dev(order)
+        self.d_pos_of = _to_dev(inverse_order(order))        # candidate mode: to-index -> sorted position
         self.packs = []
         for v in range(3):
             goff = group_word_offsets(lens[v][order])
@@ -116,11 +120,13 @@ def _call_ids(F, T, same):
     return remap(F, map_f) + remap(T, map_t) + (u_blob, u_off)
 
 
-def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift, to_index_base, k, kept=None, reuse=False):
+def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift, to_index_base, k, kept=None, reuse=False,
+             cand=None):
     """Stage the from-list (and the to-list, unless `kept` -- an editdist.KeptTargets -- holds it already and `reuse` allows
     it), join the two vocabularies, and enqueue K3b for every alphabet batch and word class: pfz_fuzz_argbest with part_*
-    [n_splits, n_from] when k is None, else pfz_fuzz_topk with part_* [n_splits, n_from, k].  Returns (part_idx, part_score,
-    n_splits, staged): `staged` keeps the staged buffers alive until the caller has synchronised."""
+    [n_splits, n_from] when k is None, else pfz_fuzz_topk with part_* [n_splits, n_from, k].  cand (a checked candidate
+    array): pfz_fuzz_cand_argbest / pfz_fuzz_cand_topk with one split.  Returns (part_idx, part_score, n_splits, staged):
+    `staged` keeps the staged buffers alive until the caller has synchronised."""
     dev = _dev()
     n_from, n_to = len(from_list), len(to_list)
     same = to_list is from_list and not to_index_base
@@ -137,7 +143,9 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
                          f"support at most {MAX_LEN}")
     f_ids, f_sig, t_ids, t_sig, d_tok_blob, d_tok_off = _call_ids(F, T, same)
     d_order, packs = targets.d_order, targets.packs
-    if n_splits is None:
+    if cand is not None:
+        n_splits = 1
+    elif n_splits is None:
         n_splits = default_splits(n_from, targets.n_grp)
     n_splits = max(1, min(int(n_splits), targets.n_grp))
     shape = (n_splits, n_from) if k is None else (n_splits, n_from, k)
@@ -165,7 +173,15 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
                 tens += [packs[v][0], packs[v][1], packs[v][2]]
             tens += [d_order, d_tok_blob, d_tok_off, part_idx, part_score, counter, None]
             arr = (ctypes.c_void_p * len(tens))(*[t.data_ptr() if t is not None else 0 for t in tens])
-            if k is None:
+            if cand is not None:
+                tail = (_p(cand), int(cand.shape[1]), _p(targets.d_pos_of))
+                if k is None:
+                    _lib.call("pfz_fuzz_cand_argbest", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer],
+                              float(score_cutoff), int(bool(exclude_self)), int(self_shift), *tail, _stream())
+                else:
+                    _lib.call("pfz_fuzz_cand_topk", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
+                              int(bool(exclude_self)), int(self_shift), *tail, int(k), _stream())
+            elif k is None:
                 _lib.call("pfz_fuzz_argbest", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
                           int(bool(exclude_self)), int(self_shift), n_splits, _stream())
             else:
@@ -220,3 +236,23 @@ def fuzz_topk(from_list, to_list, k, scorer="WRatio", score_cutoff=0.0, exclude_
     if to_index_base:
         idx = torch.where(idx >= 0, idx + int(to_index_base), idx)
     return idx, score
+
+
+def fuzz_cand_topk(from_list, to_list, cand, k, scorer="WRatio", score_cutoff=0.0, exclude_self=False, kept=None, reuse=False):
+    """The k best to-strings per from-string among its candidates cand[i] (editdist.check_candidates: device int32
+    [n_from, c], -1 = empty slot), under the scores, cutoff and key of fuzz_argbest / fuzz_topk.  k = 1 returns what
+    fuzz_argbest returns (best_idx int32[n_from], best_score float64[n_from]); k > 1 what fuzz_topk returns.  A row with no
+    candidate that passes gets (-1, 0.0); exclude_self, kept and reuse as in fuzz_argbest."""
+    k = check_top_n(k)
+    if scorer not in SCORER:
+        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
+    dev = _dev()
+    n_from, n_to = len(from_list), len(to_list)
+    cand = check_candidates(cand, n_from, n_to)
+    if n_from == 0 or n_to == 0 or cand.shape[1] == 0:
+        shape = (n_from,) if k == 1 else (n_from, k)
+        return torch.full(shape, -1, dtype=torch.int32, device=dev), torch.zeros(shape, dtype=torch.float64, device=dev)
+    part_idx, part_score, _, staged = _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, 1, 0, 0, None if k == 1 else k,
+                                               kept, reuse, cand)
+    torch.cuda.current_stream().synchronize()                  # the staged host buffers above go out of scope with this call
+    return part_idx[0], part_score[0]

@@ -32,6 +32,12 @@ CPU fallback.
 top_n = k (1..32) returns the k best to-strings per from-string (process.extract(..., limit=k) semantics: score desc, then
 to-index asc) in the columns To, Similarity, To_2, Similarity_2, ...; the reference implements top_n only for TF-IDF and
 Embeddings (polyfuzz/polyfuzz.py:100-102).  top_n = 1 is the arg-best path, unchanged.
+candidates = TFIDF(...) (new): score only each from-string's TF-IDF candidates -- `candidates.match_arrays(from_list, to_list,
+re_train)`, its top-n to-indices per row -- with this matcher's scorer, instead of every pair (blocking, DESIGN.md 4.16).  Each
+row is the all-pairs row of the same matcher against the to-strings of its candidate list (same scores, cutoff, key and
+self-exclusion), and a row without a candidate that passes is (None, 0.0), for EditDistance too; EditDistance's `normalize`
+then takes its min and max over the filled cells, as its top_n > 1 path does.  A to-string outside a row's TF-IDF top-n is
+never scored, so the best edit-distance match can be missed: that is the trade (DESIGN.md 7.16 measures it).
 Deviations from the reference, both documented reference bugs (SURVEY.md 8a): a self-match excludes
 index i only (the reference mutates the shared to_list, _rapidfuzz.py:103-104), and the matcher can be
 reused for a two-list call after a self-match (`equal_lists` is per call)."""
@@ -146,6 +152,37 @@ def _topk_frame(from_list, targets, idx, score):
     return pd.DataFrame(cols)
 
 
+def _check_candidates(candidates, top_n, distributed):
+    """The constructors' check of `candidates`: None, or a TFIDF with top_n >= the matcher's and distributed=False (the TF-IDF
+    itself may be distributed: its merged top-n is the same on every rank)."""
+    if candidates is None:
+        return None
+    from ._tfidf import TFIDF
+    if not isinstance(candidates, TFIDF):
+        raise ValueError(f"candidates must be a polyfuzz_b200.TFIDF instance, got {type(candidates).__name__}")
+    if top_n > candidates.top_n:
+        raise ValueError(f"top_n={top_n} exceeds the candidates' top_n={candidates.top_n}")
+    if distributed:
+        raise ValueError("distributed=True cannot be combined with candidates: each rank scores the few candidate pairs itself "
+                         "(pass distributed=True to the TFIDF instead)")
+    return candidates
+
+
+def _cand_topk(from_list, targets, metric, cutoff, self_match, k, candidates, to_list, re_train, kept):
+    """Candidate mode: TF-IDF's device top-n of every from-string, then the k best of those under the matcher's scorer.
+    Returns host (idx int32[n, k], -1 = empty slot, score float64[n, k])."""
+    cand, _, _ = candidates.match_arrays(from_list, to_list, re_train)
+    token_scorer = metric in fuzzy.SCORER and metric != "ratio"
+    if token_scorer:
+        idx, score = fuzzy.fuzz_cand_topk(from_list, targets, cand, k, metric, cutoff, exclude_self=self_match, kept=kept,
+                                          reuse=not re_train)
+    else:
+        idx, score = editdist.edit_cand_topk(from_list, targets, cand, k, metric, cutoff, exclude_self=self_match, kept=kept,
+                                             reuse=not re_train)[:2]
+    idx = idx.cpu().numpy(); score = score.cpu().numpy()
+    return (idx[:, None], score[:, None]) if k == 1 else (idx, score)
+
+
 def torch_full_like_int(t):
     import torch
     return torch.full_like(t, -1)
@@ -174,12 +211,14 @@ class _KeepsTargets:
 class RapidFuzz(_KeepsTargets, BaseMatcher):
     """Edit-distance matcher (GPU).  Arguments as in the reference: n_jobs (accepted, ignored -- the GPU
     scores all pairs in one launch), score_cutoff in [0,1], scorer (default fuzz.WRatio, as the reference), model_id.
-    top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given."""
+    top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given.
+    candidates (a TFIDF, top_n >= this top_n): score only its candidates per from-string (see the module docstring)."""
 
     def __init__(self, n_jobs: int = 1, score_cutoff: float = 0, scorer: Union[str, Callable] = "WRatio", model_id: str = None,
-                 distributed: bool = False, top_n: int = 1):
+                 distributed: bool = False, top_n: int = 1, candidates=None):
         super().__init__(model_id)
         self.top_n = editdist.check_top_n(top_n)
+        self.candidates = _check_candidates(candidates, self.top_n, distributed)
         self.type = "EditDistance"
         self.distributed = distributed
         self.score_cutoff = score_cutoff * 100
@@ -199,6 +238,10 @@ class RapidFuzz(_KeepsTargets, BaseMatcher):
         scale = 1.0 if unit else 100.0
         cutoff = self.score_cutoff / 100.0 if unit else self.score_cutoff
         top_n = clip_top_n(self.top_n, to_list)
+        if getattr(self, "candidates", None) is not None:
+            idx, score = _cand_topk(from_list, targets, self._metric, cutoff, self_match, top_n, self.candidates, to_list, re_train,
+                                    self._kept())
+            return _topk_frame(from_list, targets, idx, score / scale)
         if top_n > 1:
             idx, score = _topk(from_list, targets, self._metric, cutoff, self_match, self.distributed, top_n, self._kept(), not re_train)
             return _topk_frame(from_list, targets, idx.cpu().numpy(), score.cpu().numpy() / scale)
@@ -210,6 +253,16 @@ class RapidFuzz(_KeepsTargets, BaseMatcher):
                              "Similarity": np.where(idx >= 0, score, 0.0)})
 
 
+def _normalize_filled(idx, score):
+    """EditDistance's min-max normalisation over the filled cells (idx >= 0) of a top-k frame; empty slots stay 0.0."""
+    filled = idx >= 0
+    if not filled.any():
+        return np.zeros_like(score)
+    lo, hi = score[filled].min(), score[filled].max()
+    with np.errstate(invalid="ignore", divide="ignore"):
+        return np.where(filled, (score - lo) / (hi - lo), 0.0)
+
+
 class EditDistance(_KeepsTargets, BaseMatcher):
     """Edit-distance matcher with the reference's EditDistance surface (n_jobs, scorer, model_id, normalize):
     Similarity is the scorer's raw value (fuzz.ratio: 0..100, Levenshtein / OSA / DL / Jaro / Jaro-Winkler: 0..1) of the best to-string,
@@ -217,12 +270,14 @@ class EditDistance(_KeepsTargets, BaseMatcher):
     top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given; an empty
     slot is (None, 0.0).  With top_n > 1, `normalize` takes ONE min and ONE max over every filled Similarity cell of the
     frame (empty slots excluded), so the first Similarity column can differ from the top_n = 1 frame's, whose min and max
-    cover the best matches only; without `normalize` the first three columns are the top_n = 1 frame."""
+    cover the best matches only; without `normalize` the first three columns are the top_n = 1 frame.
+    candidates (a TFIDF, top_n >= this top_n): score only its candidates per from-string (see the module docstring)."""
 
     def __init__(self, n_jobs: int = 1, scorer: Union[str, Callable] = "ratio", model_id: str = None, normalize: bool = True,
-                 distributed: bool = False, top_n: int = 1):
+                 distributed: bool = False, top_n: int = 1, candidates=None):
         super().__init__(model_id)
         self.top_n = editdist.check_top_n(top_n)
+        self.candidates = _check_candidates(candidates, self.top_n, distributed)
         self.type = "EditDistance"
         self.distributed = distributed
         self.scorer = scorer
@@ -241,15 +296,16 @@ class EditDistance(_KeepsTargets, BaseMatcher):
         # score_cutoff = 0 (their default), which every score passes
         no_cut = 0.0 if self._metric in fuzzy.SCORER and self._metric != "ratio" else float("-inf")
         top_n = clip_top_n(self.top_n, to_list)
-        if top_n > 1:
-            idx, score = _topk(from_list, targets, self._metric, no_cut, self_match, self.distributed, top_n, self._kept(), not re_train)
-            idx = idx.cpu().numpy(); score = score.cpu().numpy()
-            if self.normalize:
-                filled = idx >= 0
-                lo, hi = score[filled].min(), score[filled].max()
-                with np.errstate(invalid="ignore", divide="ignore"):
-                    score = np.where(filled, (score - lo) / (hi - lo), 0.0)
-            return _topk_frame(from_list, targets, idx, score)
+        cand = getattr(self, "candidates", None) is not None
+        if top_n > 1 or cand:
+            if cand:
+                idx, score = _cand_topk(from_list, targets, self._metric, no_cut, self_match, top_n, self.candidates, to_list,
+                                        re_train, self._kept())
+            else:
+                idx, score = _topk(from_list, targets, self._metric, no_cut, self_match, self.distributed, top_n, self._kept(),
+                                   not re_train)
+                idx = idx.cpu().numpy(); score = score.cpu().numpy()
+            return _topk_frame(from_list, targets, idx, _normalize_filled(idx, score) if self.normalize else score)
         idx, score, _ = _argbest(from_list, targets, self._metric, no_cut, self_match, self.distributed, self._kept(), not re_train)
         idx = idx.cpu().numpy(); score = score.cpu().numpy()
         to_arr = np.empty(len(targets), dtype=object); to_arr[:] = targets
