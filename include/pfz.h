@@ -39,8 +39,8 @@ extern "C" {
 #define PFZ_METRIC_JARO_WINKLER 5  /* jellyfish jaro_winkler_similarity(from, to), long_tolerance=False */
 #define PFZ_METRIC_OSA       6     /* optimal string alignment distance (restricted Damerau-Levenshtein) */
 #define PFZ_METRIC_NORM_OSA  7     /* 1 - osa/max(|a|,|b|)                                         */
-#define PFZ_METRIC_DL        8     /* unrestricted Damerau-Levenshtein distance (pfz_dl_* only)    */
-#define PFZ_METRIC_NORM_DL   9     /* 1 - dl/max(|a|,|b|)                   (pfz_dl_* only)        */
+#define PFZ_METRIC_DL        8     /* unrestricted Damerau-Levenshtein distance                    */
+#define PFZ_METRIC_NORM_DL   9     /* 1 - dl/max(|a|,|b|)                                          */
 
 int         pfz_abi_version(void);
 const char *pfz_last_error(void);
@@ -228,7 +228,7 @@ int pfz_topk_merge(const int32_t *idx, const double *val, int32_t n_lists, int32
                    int32_t k_out, int32_t *out_idx, double *out_val, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
- * K3  all-pairs edit distance with a fused per-row arg-best.
+ * K3  edit distance, all pairs or per-row candidate lists, with a fused per-row arg-best or top-k.
  * Replaces: rapidfuzz process.extractOne / scorer loops as called at polyfuzz/models/_rapidfuzz.py:99-113
  *           and polyfuzz/models/_distance.py:89-102 (np.argmax = first maximum).
  * Symbols are bytes: sym_table (uint8[0x110000]) maps the code points of the from-strings to 1..255
@@ -241,104 +241,53 @@ int pfz_topk_merge(const int32_t *idx, const double *val, int32_t n_lists, int32
 int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32_t *order, int32_t n_to,
                  const uint8_t *sym_table, const int64_t *grp_word_off, uint32_t *packed, int32_t *slen, void *stream);
 
-/* scores the from-strings listed in from_ids (all of one word class: n_words = 0 -> length <= 32 (one
- * 32-bit word), 1/2/4/8/16 -> length <= 64*n_words) against every to-string.
- *   metric: PFZ_METRIC_*; for NORM_LEV / JARO / JARO_WINKLER / NORM_OSA a candidate needs score >= score_cutoff; for RATIO
+/* Scores the from-strings listed in from_ids (all of one word class: n_words = 0 -> length <= 32 (one 32-bit word),
+ * 1/2/4/8/16 -> length <= 64*n_words) against the to-strings, with a fused per-row epilogue.
+ * Replaces: rapidfuzz process.extractOne / process.extract(query, to_list, scorer, limit=k) and the scorer loop of
+ *           polyfuzz/models/_distance.py:98-99 (np.argmax, or the sort of the scorer values for top-k).
+ *   metric: PFZ_METRIC_*; for NORM_LEV / JARO / JARO_WINKLER / NORM_OSA / NORM_DL a candidate needs score >= score_cutoff; for RATIO
  *           rapidfuzz's two steps: ns = 1 - indel/(|a|+|b|) >= score_cutoff/100 (fuzz.ratio) and score = ns*100 >= score_cutoff
- *           (extractOne), which differ whenever (ns*100)/100 != ns -- e.g. ns = 17/25 is rejected at score_cutoff 68.0
+ *           (extractOne), which differ whenever (ns*100)/100 != ns -- e.g. ns = 17/25 is rejected at score_cutoff 68.0; the raw
+ *           distances LEV, INDEL, OSA and DL have no cutoff (best = smallest)
  *   exclude_self: skip to-row == from-row + self_shift
- *   part_*: [n_splits][n_from] partial bests (merge with pfz_lev_merge); ties -> lowest to-index;
- *           part_dist holds the distance, or for JARO / JARO_WINKLER the number of matching characters
- *   matrix (may be NULL): int32 [n_from][matrix_ld] full distance matrix (Levenshtein, Indel, or OSA for OSA /
- *           NORM_OSA); must be NULL for JARO / JARO_WINKLER
- * OSA / NORM_OSA: optimal string alignment (restricted Damerau-Levenshtein) on code points: insertions, deletions,
- * substitutions and swaps of two adjacent characters, no substring edited twice (osa("CA", "ABC") = 3, where unrestricted
- * Damerau-Levenshtein gives 2); DESIGN.md 4.9 gives the recurrence.
+ *   key: score desc, to-index asc (ties -> lowest to-index)
+ *   k (epilogue): 0 = arg-best: part_idx / part_score / part_dist [n_splits][n_from] partial bests (merge with pfz_lev_merge);
+ *           part_dist holds the distance, or for JARO / JARO_WINKLER the number of matching characters; empty (-1, 0.0, -1).
+ *           1..32 = top-k: part_idx / part_score [n_splits][n_from][k] sorted lists, empty slots (-1, 0.0) (merge with
+ *           pfz_topk_merge); metric NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA or NORM_DL; part_dist and matrix NULL.
+ *   matrix (arg-best, may be NULL): int32 [n_from][matrix_ld] full distance matrix (Levenshtein, Indel, OSA for OSA / NORM_OSA, DL
+ *           for DL / NORM_DL); must be NULL for JARO / JARO_WINKLER, and needs gate == NULL
+ *   gate (DL / NORM_DL only, may be NULL): float64[n_from], per from-row a proven lower bound of its k-th best score (k = 1 for the
+ *           arg-best) over the row's to-strings; pairs whose score upper bound is below it are skipped.  The k-th best OSA score of
+ *           the row (this call with OSA / NORM_OSA and the same cutoff, exclusion and k, merged over the splits) is such a bound,
+ *           and a row with fewer than k OSA candidates takes score_cutoff (NORM_DL) or -inf (DL).  NULL: no gate.
  *   counter: int32[n_splits], zeroed by the callee
+ *   cand_idx (source): NULL = all pairs, the to-list split over n_splits >= 1.  Non-NULL = candidate mode: each from-row scores
+ *           only its own list, e.g. TF-IDF's top-n for that row (the blocking step users run around the reference); n_splits = 1,
+ *           cand_idx int32[n_from][c] (c >= 1) to-indices per from-row, distinct within a row, -1 = empty slot (TF-IDF's top_idx);
+ *           pos_of int32[n_to] the sorted position of each to-index (the inverse of pfz_lev_pack's `order`).  part_* are then the
+ *           outputs, one list per row, no merge.  A row's result is that of all pairs against the to-strings of its list, bit for
+ *           bit; matrix: only the candidate pairs' cells are written; gate: a bound over the row's candidates.
+ * OSA / NORM_OSA: optimal string alignment (restricted Damerau-Levenshtein) on code points: insertions, deletions,
+ * substitutions and swaps of two adjacent characters, no substring edited twice (osa("CA", "ABC") = 3); DESIGN.md 4.9 gives the
+ * recurrence.  DL / NORM_DL: unrestricted Damerau-Levenshtein (Lowrance-Wagner with unit costs, on code points), where a swapped
+ * pair may be edited again (dl("CA", "ABC") = 2); NORM_DL = 1 - dl/max(|a|,|b|); DESIGN.md 4.10 gives the bounds and the kernel.
  * JARO / JARO_WINKLER: jellyfish's definition on code points, from-string first (the reference calls
- * scorer(from_string, to_string), polyfuzz/models/_distance.py:98); DESIGN.md 4.5 gives the recurrence.  */
-int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                    int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                    const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                    int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
-                    int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
-                    int32_t *counter, void *stream);
+ * scorer(from_string, to_string), polyfuzz/models/_distance.py:98); DESIGN.md 4.5 gives the recurrence.
+ * n_ids <= 0 (or n_to < 0) returns 0 without launching anything.                                                          */
+int pfz_lev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                 int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off,
+                 const int32_t *slen, const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff,
+                 int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k,
+                 const int32_t *cand_idx, int32_t c, const int32_t *pos_of,
+                 int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
+                 const double *gate, int32_t *counter, void *stream);
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits,
                   int32_t n_from, int32_t *best_idx, double *best_score, int32_t *best_dist, void *stream);
 
-/* top-k sibling of pfz_lev_argbest: the k best to-strings per from-string (1 <= k <= 32), same candidates (the cutoff tests
- * above, to-row == from-row + self_shift excluded when exclude_self) and key (score desc, to-index asc).
- * Replaces: rapidfuzz process.extract(query, to_list, scorer, limit=k), and the sort of the scorer values of
- *           polyfuzz/models/_distance.py:98-99 where the reference takes np.argmax.
- *   metric: NORM_LEV, RATIO, JARO, JARO_WINKLER or NORM_OSA; there is no distance output and no matrix.
- *   part_idx / part_score: [n_splits][n_from][k] sorted lists, empty slots (-1, 0.0); merge them with pfz_topk_merge.   */
-int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                 int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                 const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                 int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
-                 int32_t k, int32_t *part_idx, double *part_score, int32_t *counter, void *stream);
-
-/* Unrestricted Damerau-Levenshtein (Lowrance-Wagner with unit costs, on code points): the fewest insertions, deletions,
- * substitutions and swaps of two adjacent characters, where a swapped pair may be edited again (dl("CA", "ABC") = 2).
- * Same parameters, layout, candidates, key and outputs as pfz_lev_argbest / pfz_lev_topk, plus
- *   gate (may be NULL): float64[n_from], per from-row a proven lower bound of its k-th best score (k = 1 for the arg-best) over
- *         the whole to-list; pairs whose score upper bound is below it are skipped.  The k-th best OSA score of the row (the
- *         pfz_lev_* pass with OSA / NORM_OSA and the same cutoff, exclusion and k, merged over the splits) is such a bound, and a
- *         row with fewer than k OSA candidates takes score_cutoff (NORM_DL) or -inf (DL).  NULL: no gate.
- *   metric: DL (raw distance, best = smallest, no cutoff; arg-best only) or NORM_DL (1 - dl/max(|a|,|b|), score >= score_cutoff).
- *   matrix (arg-best only, may be NULL): DL distances of every pair; requires gate == NULL.
- * DESIGN.md 4.10 gives the bounds and the kernel. */
-int pfz_dl_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                   int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                   const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                   int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
-                   int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
-                   const double *gate, int32_t *counter, void *stream);
-int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
-                int32_t k, int32_t *part_idx, double *part_score, const double *gate, int32_t *counter, void *stream);
-
-/* Candidate mode of K3: each from-row scores only its own list of to-strings, e.g. TF-IDF's top-n for that row.
- * Replaces: the blocking step users run around the reference -- TF-IDF's top-n per from-string, then rapidfuzz's
- *           process.extractOne / process.extract(query, [to_list[j] for j in candidates], scorer, ...) (the scorer loop of
- *           polyfuzz/models/_rapidfuzz.py:99-113 and polyfuzz/models/_distance.py:89-102 restricted to those pairs).
- * Same parameters, metrics, cutoffs, self-exclusion, key and kernels as the all-pairs sibling, without n_splits, plus
- *   cand_idx: int32[n_from][c] to-indices per from-row, distinct within a row, -1 = empty slot (TF-IDF's top_idx)
- *   pos_of:   int32[n_to] the sorted position of each to-index (the inverse of pfz_lev_pack's `order`)
- * Outputs: one list per row, no merge -- best_* int32 / float64 / int32 [n_from] (argbest; (-1, 0.0, -1) for a row with no
- * candidate that passes), top_* [n_from][k] (topk; empty slots (-1, 0.0)).  A row's result is that of the all-pairs entry
- * point against the to-strings of its list, bit for bit.  matrix (argbest, may be NULL): only the candidate pairs' cells are
- * written.  gate (DL, may be NULL): a lower bound of the row's k-th best score over its candidates.  counter: int32[1]. */
-int pfz_lev_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                         int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                         const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                         int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                         const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
-                         int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, int32_t *counter, void *stream);
-int pfz_lev_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                      int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                      const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                      int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                      const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
-                      int32_t *counter, void *stream);
-int pfz_dl_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                        int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                        const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                        int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                        const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
-                        int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream);
-int pfz_dl_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                     int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed,
-                     const int64_t *grp_word_off, const int32_t *slen, const int32_t *sorig, int32_t n_to,
-                     int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                     const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
-                     const double *gate, int32_t *counter, void *stream);
-
-/* K3b  rapidfuzz's token / partial / weighted scorers with a fused per-row arg-best (csrc/pfz_fuzz.cu).
- * Replaces: process.extractOne(query, to_list, scorer=fuzz.WRatio | partial_ratio | token_*_ratio | ..., score_cutoff) at
- *           polyfuzz/models/_rapidfuzz.py:48,106-108 and the scorer loop of polyfuzz/models/_distance.py:98.
+/* K3b  rapidfuzz's token / partial / weighted scorers with a fused per-row epilogue (csrc/pfz_fuzz.cu).
+ * Replaces: process.extractOne / process.extract(query, to_list, scorer=fuzz.WRatio | partial_ratio | token_*_ratio | ...,
+ *           score_cutoff, limit=k) at polyfuzz/models/_rapidfuzz.py:48,106-108 and the scorer loop of polyfuzz/models/_distance.py:98.
  * scorer: 0 ratio, 1 QRatio, 2 partial_ratio, 3 token_sort_ratio, 4 token_set_ratio, 5 token_ratio, 6 partial_token_sort_ratio,
  *         7 partial_token_set_ratio, 8 partial_token_ratio, 9 WRatio (rapidfuzz 3.x definitions, processor=None; scores 0..100).
  * ptrs: 38 device pointers -- for the from-side then the to-side: {blob uint32, offsets int64} of s, S(s) = sorted tokens
@@ -348,15 +297,21 @@ int pfz_dl_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int
  *       8, 16 for from-strings whose longest variant has up to 64, 128, 256, 512, 1024 code points; to-strings of any
  *       length), sym_table uint8[0x110000], for each variant {packed, grp_word_off, slen}
  *       (pfz_lev_pack layouts of b, S(b), U(b) in ONE length order), sorig int32[n_to], tok_blob uint32, tok_off int64[n_tok+1],
- *       part_idx int32[n_splits][n_from], part_score float64[n_splits][n_from], counter int32[n_splits], reserved (NULL).
- * Best = first to-string (lowest index) with the maximal score >= score_cutoff; merge the splits with pfz_lev_merge.
+ *       part_idx, part_score, counter int32[n_splits], reserved (NULL).
+ * k (epilogue): 0 = arg-best: part_idx int32 / part_score float64 [n_splits][n_from], best = first to-string (lowest index) with
+ *       the maximal score >= score_cutoff; merge the splits with pfz_lev_merge.  1..32 = top-k: [n_splits][n_from][k] sorted lists
+ *       under the same candidates and key (score desc, to-index asc), empty slots (-1, 0.0); merge them with pfz_topk_merge.
+ * cand_idx (source): NULL = all pairs over n_splits >= 1 splits; non-NULL = candidate mode as in pfz_lev_rows (n_splits = 1,
+ *       cand_idx int32[n_from][c] with c >= 1, pos_of int32[n_to], part_* the outputs, no merge).
  * The cutoff reaches the scorer as in rapidfuzz: ratio (also inside token_sort_ratio, token_ratio, QRatio, WRatio) keeps
  * ns = 1 - indel/(|a|+|b|) only if ns >= score_cutoff/100, and partial_ratio (also inside the partial_token_* scorers and
  * WRatio) keeps its best window's ns only if ns >= score_cutoff/100 and ns*100 >= score_cutoff; the token-set parts test
  * 100 - 100*dist/lensum >= score_cutoff once.  So a pair is rejected at a cutoff equal to its own score whenever
- * (ns*100)/100 > ns in doubles, and WRatio's internal cutoffs (max(c, end_ratio)/0.9, /0.95) apply the same rule.          */
-int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
-                     int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream);
+ * (ns*100)/100 > ns in doubles, and WRatio's internal cutoffs (max(c, end_ratio)/0.9, /0.95) apply the same rule.
+ * n_ids <= 0 or n_to <= 0 returns 0 without launching anything.                                                           */
+int pfz_fuzz_rows(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
+                  int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k,
+                  const int32_t *cand_idx, int32_t c, const int32_t *pos_of, void *stream);
 
 /* K3b's token tables, built on the device (csrc/pfz_tok.cu).  Replaces the host derivation of s.split(), sorted(), the token
  * dictionary and the signatures.  Tokens are Python str.split()'s: maximal runs of code points c with not chr(c).isspace().
@@ -381,27 +336,6 @@ int pfz_tok_union(const int32_t *a_blob, const int64_t *a_off, int32_t n_a, cons
                   int32_t *map_a, int32_t *map_b, int32_t *u_blob, int64_t *u_off, int32_t *n_u, void *stream);
 int pfz_tok_remap(const int32_t *tok_ptr, const int32_t *ids_in, int32_t n, const int32_t *map, int32_t *ids_out, uint64_t *sig,
                   void *stream);
-
-/* top-k sibling of pfz_fuzz_argbest: the k best to-strings per from-string (1 <= k <= 32) under the same candidates and key.
- * Replaces: rapidfuzz process.extract(query, to_list, scorer=..., score_cutoff=..., limit=k), and the sort of the scorer values
- *           of polyfuzz/models/_distance.py:98-99 where the reference takes np.argmax.
- * ptrs: as pfz_fuzz_argbest, except part_idx int32 / part_score float64 are [n_splits][n_from][k] sorted lists with empty slots
- *       (-1, 0.0); merge them with pfz_topk_merge.                                                                               */
-int pfz_fuzz_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
-                  int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k,
-                  void *stream);
-
-/* Candidate mode of K3b (see pfz_lev_cand_argbest): the siblings' scorers, cutoffs and key over each from-row's own list.
- * Replaces: process.extractOne / process.extract(query, [to_list[j] for j in candidates], scorer=fuzz.WRatio | ..., ...) --
- *           the reference's RapidFuzz scorer loop (polyfuzz/models/_rapidfuzz.py:106-108) over a blocked candidate set.
- * ptrs: as pfz_fuzz_argbest, except part_idx / part_score are the outputs: [n_from] (argbest) or [n_from][k] (topk);
- * cand_idx int32[n_from][c] and pos_of int32[n_to] as in pfz_lev_cand_argbest; counter int32[1].                            */
-int pfz_fuzz_cand_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
-                          int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
-                          int32_t c, const int32_t *pos_of, void *stream);
-int pfz_fuzz_cand_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
-                       int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
-                       int32_t c, const int32_t *pos_of, int32_t k, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K4  dense cosine top-k for pre-computed embeddings (bf16 wgmma GEMM fed by TMA, top-k fused into the

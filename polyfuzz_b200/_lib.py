@@ -40,27 +40,10 @@ _PROTOS = {
     "pfz_spcos_topk_block": [c_vp, c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32,
                              c_i64, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_lev_pack": [c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp],
-    "pfz_lev_argbest": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                        c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp],
+    "pfz_lev_rows": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64, c_i32,
+                     c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp],
     "pfz_lev_merge": [c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp],
-    "pfz_fuzz_argbest": [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i32, c_vp],
-    "pfz_lev_topk": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                     c_i32, c_i32, c_vp, c_vp, c_vp, c_vp],
-    "pfz_dl_argbest": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                       c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp],
-    "pfz_dl_topk": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                    c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp],
-    "pfz_fuzz_topk":[c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i32, c_i32, c_vp],
-    "pfz_lev_cand_argbest": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                             c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp],
-    "pfz_lev_cand_topk": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                          c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp],
-    "pfz_dl_cand_argbest": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                            c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp],
-    "pfz_dl_cand_topk": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64,
-                         c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp],
-    "pfz_fuzz_cand_argbest": [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_vp, c_i32, c_vp, c_vp],
-    "pfz_fuzz_cand_topk": [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_vp, c_i32, c_vp, c_i32, c_vp],
+    "pfz_fuzz_rows": [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp],
     "pfz_tok_side": [c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_tok_union": [c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_tok_remap": [c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp],

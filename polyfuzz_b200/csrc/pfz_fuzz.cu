@@ -445,30 +445,9 @@ static int launch_fuzz(const FuzzParams &P, int sms, cudaStream_t st) {
     }
 }
 
-// the 38 pointers of the C ABI (order: include/pfz.h) -> FuzzParams; part_idx / part_score as the caller's entry point lays them out.
-// CAND: the candidate entry points (cl: the rows' lists, n_splits = 1).
-template <bool TOPK, bool CAND = false>
-static int run_fuzz(const void *const *ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
-                    double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k_out, void *stream,
-                    const CandList &cl = CandList{nullptr, 0, nullptr}) {
-    cudaStream_t st = as_stream(stream);
-    FuzzParams P;
-    int k = 0;
-    auto side = [&](FuzzSide &S) {
-        for (int v = 0; v < 3; ++v) { S.blob[v] = (const uint32_t *)ptrs[k++]; S.off[v] = (const int64_t *)ptrs[k++]; }
-        S.tok_ptr = (const int32_t *)ptrs[k++]; S.tok_ids = (const int32_t *)ptrs[k++]; S.sig = (const uint64_t *)ptrs[k++];
-        S.n_tok_all = (const int32_t *)ptrs[k++];
-    };
-    side(P.F); side(P.T);                                                           // 2 x 10
-    P.from_ids = (const int32_t *)ptrs[k++]; P.sym_table = (const uint8_t *)ptrs[k++];   // 22
-    for (int v = 0; v < 3; ++v) { P.packed[v] = (const uint32_t *)ptrs[k++]; P.grp_off[v] = (const int64_t *)ptrs[k++]; P.slen[v] = (const int32_t *)ptrs[k++]; }   // 31
-    P.sorig = (const int32_t *)ptrs[k++]; P.tok_blob = (const uint32_t *)ptrs[k++]; P.tok_off = (const int64_t *)ptrs[k++];     // 34
-    P.part_idx = (int32_t *)ptrs[k++]; P.part_score = (double *)ptrs[k++]; P.counter = (int32_t *)ptrs[k++];                  // 37
-    k++;                                                                            // 38: reserved
-    P.n_ids = n_ids; P.n_to = n_to; P.scorer = scorer; P.cutoff = score_cutoff; P.exclude_self = exclude_self; P.self_shift = self_shift;
-    P.n_splits = n_splits; P.n_from = n_from; P.k = k_out; P.cand = cl;
-    int sms = 0;
-    if (start_rows(P.counter, n_splits, st, &sms)) return 1;
+// n_words (1, 2, 4, 8, 16) -> launch_fuzz<NW>
+template <bool TOPK, bool CAND>
+static int launch_words(const FuzzParams &P, int n_words, int sms, cudaStream_t st) {
     if (n_words == 1) return launch_fuzz<1, TOPK, CAND>(P, sms, st);
     if (n_words == 2) return launch_fuzz<2, TOPK, CAND>(P, sms, st);
     if (n_words == 4) return launch_fuzz<4, TOPK, CAND>(P, sms, st);
@@ -482,59 +461,41 @@ using namespace pfz;
 
 extern "C" {
 
-/* ptrs: 38 device pointers in the order of PfzFuzzArgs below (one flat array keeps the C ABI free of structs) */
-int pfz_fuzz_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
-                     double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, void *stream) {
-    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_argbest: expected 38 pointers, got %d", n_ptrs);
-    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_argbest: unknown scorer %d", scorer);
+// Every rule on n_ptrs, the scorer, the epilogue (k) and the source (cand_idx) is checked first, before any CUDA call; then the
+// 38 pointers (order: include/pfz.h) become FuzzParams, the row counters are zeroed and the <NW, TOPK, CAND> instantiation runs.
+int pfz_fuzz_rows(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
+                  double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k, const int32_t *cand_idx,
+                  int32_t c, const int32_t *pos_of, void *stream) {
+    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_rows: expected 38 pointers, got %d", n_ptrs);
+    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_rows: unknown scorer %d", scorer);
     PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_fuzz_argbest: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
-    PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_argbest: n_splits < 1");
+                "pfz_fuzz_rows: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
+    PFZ_REQUIRE(k >= 0 && k <= 32, "pfz_fuzz_rows: k=%d unsupported (0 = arg-best, 1..32 = top-k)", k);
+    if (cand_idx)
+        PFZ_REQUIRE(n_splits == 1 && c >= 1 && pos_of, "pfz_fuzz_rows: candidate mode needs n_splits = 1, c >= 1 and pos_of "
+                    "(n_splits=%d, c=%d, pos_of %p)", n_splits, c, (const void *)pos_of);
+    else
+        PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_rows: n_splits < 1");
     if (n_ids <= 0 || n_to <= 0) return 0;
-    return run_fuzz<false>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, n_splits, 1, stream);
-}
-
-/* ptrs: as pfz_fuzz_argbest, with part_idx / part_score laid out [n_splits][n_from][k] */
-int pfz_fuzz_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to, int32_t scorer,
-                  double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k, void *stream) {
-    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_topk: expected 38 pointers, got %d", n_ptrs);
-    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_topk: unknown scorer %d", scorer);
-    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_fuzz_topk: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
-    PFZ_REQUIRE(n_splits >= 1, "pfz_fuzz_topk: n_splits < 1");
-    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_fuzz_topk: k=%d unsupported (1..32)", k);
-    if (n_ids <= 0 || n_to <= 0) return 0;
-    return run_fuzz<true>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, n_splits, k, stream);
-}
-
-/* ptrs: as pfz_fuzz_argbest, with part_idx / part_score the outputs best_idx int32[n_from] / best_score float64[n_from] */
-int pfz_fuzz_cand_argbest(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
-                          int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
-                          int32_t c, const int32_t *pos_of, void *stream) {
-    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_cand_argbest: expected 38 pointers, got %d", n_ptrs);
-    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_cand_argbest: unknown scorer %d", scorer);
-    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_fuzz_cand_argbest: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
-    PFZ_REQUIRE(c >= 0 && (c == 0 || (cand_idx && pos_of)), "pfz_fuzz_cand_argbest: c=%d with cand_idx %p, pos_of %p", c,
-                (const void *)cand_idx, (const void *)pos_of);
-    if (n_ids <= 0 || n_to <= 0) return 0;
-    return run_fuzz<false, true>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, 1, 1, stream,
-                                 CandList{cand_idx, c, pos_of});
-}
-
-/* ptrs: as pfz_fuzz_argbest, with part_idx / part_score the outputs top_idx int32[n_from][k] / top_score float64[n_from][k] */
-int pfz_fuzz_cand_topk(const void *const *ptrs, int32_t n_ptrs, int32_t n_from, int32_t n_ids, int32_t n_words, int32_t n_to,
-                       int32_t scorer, double score_cutoff, int32_t exclude_self, int64_t self_shift, const int32_t *cand_idx,
-                       int32_t c, const int32_t *pos_of, int32_t k, void *stream) {
-    PFZ_REQUIRE(n_ptrs == 38, "pfz_fuzz_cand_topk: expected 38 pointers, got %d", n_ptrs);
-    PFZ_REQUIRE(scorer >= FZ_RATIO && scorer <= FZ_WRATIO, "pfz_fuzz_cand_topk: unknown scorer %d", scorer);
-    PFZ_REQUIRE(n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "pfz_fuzz_cand_topk: n_words %d unsupported (1, 2, 4, 8, 16: from-strings up to 1024 code points)", n_words);
-    PFZ_REQUIRE(c >= 0 && (c == 0 || (cand_idx && pos_of)), "pfz_fuzz_cand_topk: c=%d with cand_idx %p, pos_of %p", c,
-                (const void *)cand_idx, (const void *)pos_of);
-    PFZ_REQUIRE(k >= 1 && k <= 32, "pfz_fuzz_cand_topk: k=%d unsupported (1..32)", k);
-    if (n_ids <= 0 || n_to <= 0) return 0;
-    return run_fuzz<true, true>(ptrs, n_from, n_ids, n_words, n_to, scorer, score_cutoff, exclude_self, self_shift, 1, k, stream,
-                                CandList{cand_idx, c, pos_of});
+    cudaStream_t st = as_stream(stream);
+    FuzzParams P;
+    int q = 0;
+    auto side = [&](FuzzSide &S) {
+        for (int v = 0; v < 3; ++v) { S.blob[v] = (const uint32_t *)ptrs[q++]; S.off[v] = (const int64_t *)ptrs[q++]; }
+        S.tok_ptr = (const int32_t *)ptrs[q++]; S.tok_ids = (const int32_t *)ptrs[q++]; S.sig = (const uint64_t *)ptrs[q++];
+        S.n_tok_all = (const int32_t *)ptrs[q++];
+    };
+    side(P.F); side(P.T);                                                           // 2 x 10
+    P.from_ids = (const int32_t *)ptrs[q++]; P.sym_table = (const uint8_t *)ptrs[q++];   // 22
+    for (int v = 0; v < 3; ++v) { P.packed[v] = (const uint32_t *)ptrs[q++]; P.grp_off[v] = (const int64_t *)ptrs[q++]; P.slen[v] = (const int32_t *)ptrs[q++]; }   // 31
+    P.sorig = (const int32_t *)ptrs[q++]; P.tok_blob = (const uint32_t *)ptrs[q++]; P.tok_off = (const int64_t *)ptrs[q++];     // 34
+    P.part_idx = (int32_t *)ptrs[q++]; P.part_score = (double *)ptrs[q++]; P.counter = (int32_t *)ptrs[q++];                  // 37
+    q++;                                                                            // 38: reserved
+    P.n_ids = n_ids; P.n_to = n_to; P.scorer = scorer; P.cutoff = score_cutoff; P.exclude_self = exclude_self; P.self_shift = self_shift;
+    P.n_splits = n_splits; P.n_from = n_from; P.k = k; P.cand = CandList{cand_idx, c, pos_of};
+    int sms = 0;
+    if (start_rows(P.counter, n_splits, st, &sms)) return 1;
+    if (cand_idx) return k ? launch_words<true, true>(P, n_words, sms, st) : launch_words<false, true>(P, n_words, sms, st);
+    return k ? launch_words<true, false>(P, n_words, sms, st) : launch_words<false, false>(P, n_words, sms, st);
 }
 }

@@ -17,7 +17,7 @@
 //
 // Shared by the kernels here: the row driver of pfz_common.cuh (split_groups, claim_row, build_peq, WarpArgBest / WarpTopK,
 // launch_rows), LevColumn (the Levenshtein / OSA column step of lev_kernel and dl_kernel), for_each_text_symbol (the text
-// loop), dispatch_words (n_words -> <W, NW>) and run_k3 (the body of the C entry points).
+// loop), dispatch_words (n_words -> <W, NW>) and launch_class (the metric -> kernel choice of pfz_lev_rows).
 #include "pfz_common.cuh"
 #include <math_constants.h>
 #include <cmath>
@@ -645,31 +645,6 @@ static int launch_class(const LevParams &P, const double *gate, int n_words, int
     });
 }
 
-// The body of the K3 entry points after their metric checks: the checks they share, the row counters and the launch.
-// fn names the entry point in error messages.  CAND: the candidate entry points (cl: the rows' lists, n_splits = 1).
-template <bool TOPK, bool CAND = false>
-static int run_k3(const char *fn, const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids,
-                  int32_t n_ids, int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off,
-                  const int32_t *slen, const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self,
-                  int64_t self_shift, int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, int32_t *part_dist,
-                  int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream,
-                  const CandList &cl = CandList{nullptr, 0, nullptr}) {
-    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
-                "%s: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", fn, n_words);
-    PFZ_REQUIRE(n_splits >= 1, "%s: n_splits < 1", fn);
-    PFZ_REQUIRE(!TOPK || (k >= 1 && k <= 32), "%s: k=%d unsupported (1..32)", fn, k);
-    PFZ_REQUIRE(!CAND || (cl.c >= 0 && (cl.c == 0 || (cl.idx && cl.pos_of))), "%s: c=%d with cand_idx %p, pos_of %p", fn, cl.c,
-                (const void *)cl.idx, (const void *)cl.pos_of);
-    if (n_ids <= 0 || n_to < 0) return 0;
-    cudaStream_t st = as_stream(stream);
-    int sms = 0;
-    if (start_rows(counter, n_splits, st, &sms)) return 1;
-    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
-                exclude_self, self_shift, ratio_min_ns_of(score_cutoff), n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from,
-                counter, k, cl};
-    return launch_class<TOPK, CAND>(P, gate, n_words, sms, st);
-}
-
 }  // namespace pfz
 
 using namespace pfz;
@@ -686,98 +661,45 @@ int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32
     return 0;
 }
 
-int pfz_lev_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
-                    int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
-                    const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                    int32_t n_splits, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
-                    int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_OSA, "pfz_lev_argbest: unknown metric %d", metric);
-    const bool jaro = metric == PFZ_METRIC_JARO || metric == PFZ_METRIC_JARO_WINKLER;
-    PFZ_REQUIRE(!(jaro && matrix), "pfz_lev_argbest: the distance matrix is not available for the Jaro metrics (matrix must be NULL)");
-    return run_k3<false>("pfz_lev_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
-                         slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, 1, part_idx, part_score, part_dist,
-                         matrix, matrix_ld, nullptr, counter, stream);
-}
-
-int pfz_lev_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+// Every rule on the metric, the epilogue (k), the source (cand_idx), the matrix and the gate is checked first, before any CUDA
+// call; then the row counters are zeroed and the <TOPK, CAND> instantiation for (k >= 1, cand_idx != NULL) runs.
+int pfz_lev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
                  int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
                  const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                 int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, int32_t *counter, void *stream) {
-    PFZ_REQUIRE((metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER) || metric == PFZ_METRIC_NORM_OSA,
-                "pfz_lev_topk: metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA)", metric);
-    return run_k3<true>("pfz_lev_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
-                        slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, k, part_idx, part_score, nullptr,
-                        nullptr, 0, nullptr, counter, stream);
-}
-
-int pfz_dl_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
-                   int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
-                   const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                   int32_t n_splits, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld,
-                   const double *gate, int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric == PFZ_METRIC_DL || metric == PFZ_METRIC_NORM_DL, "pfz_dl_argbest: metric %d unsupported (DL, NORM_DL)", metric);
-    PFZ_REQUIRE(!(matrix && gate), "pfz_dl_argbest: the distance matrix needs every pair, so gate must be NULL with a matrix");
-    return run_k3<false>("pfz_dl_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
-                         slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, 1, part_idx, part_score, part_dist,
-                         matrix, matrix_ld, gate, counter, stream);
-}
-
-int pfz_dl_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
-                int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
-                const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                int32_t n_splits, int32_t k, int32_t *part_idx, double *part_score, const double *gate, int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric == PFZ_METRIC_NORM_DL, "pfz_dl_topk: metric %d unsupported (NORM_DL)", metric);
-    return run_k3<true>("pfz_dl_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed, grp_word_off,
-                        slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, n_splits, k, part_idx, part_score, nullptr,
-                        nullptr, 0, gate, counter, stream);
-}
-
-int pfz_lev_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
-                         int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
-                         const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                         const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
-                         int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_OSA, "pfz_lev_cand_argbest: unknown metric %d", metric);
+                 int32_t n_splits, int32_t k, const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *part_idx,
+                 double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter,
+                 void *stream) {
+    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_DL, "pfz_lev_rows: unknown metric %d", metric);
+    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_lev_rows: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
+    PFZ_REQUIRE(k >= 0 && k <= 32, "pfz_lev_rows: k=%d unsupported (0 = arg-best, 1..32 = top-k)", k);
     const bool jaro = metric == PFZ_METRIC_JARO || metric == PFZ_METRIC_JARO_WINKLER;
-    PFZ_REQUIRE(!(jaro && matrix), "pfz_lev_cand_argbest: the distance matrix is not available for the Jaro metrics (matrix must be NULL)");
-    return run_k3<false, true>("pfz_lev_cand_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
-                               grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, 1, best_idx, best_score,
-                               best_dist, matrix, matrix_ld, nullptr, counter, stream, CandList{cand_idx, c, pos_of});
-}
-
-int pfz_lev_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
-                      int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
-                      const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                      const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
-                      int32_t *counter, void *stream) {
-    PFZ_REQUIRE((metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER) || metric == PFZ_METRIC_NORM_OSA,
-                "pfz_lev_cand_topk: metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA)", metric);
-    return run_k3<true, true>("pfz_lev_cand_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
-                              grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, k, top_idx, top_score,
-                              nullptr, nullptr, 0, nullptr, counter, stream, CandList{cand_idx, c, pos_of});
-}
-
-int pfz_dl_cand_argbest(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
-                        int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
-                        const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                        const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *best_idx, double *best_score,
-                        int32_t *best_dist, int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric == PFZ_METRIC_DL || metric == PFZ_METRIC_NORM_DL, "pfz_dl_cand_argbest: metric %d unsupported (DL, NORM_DL)", metric);
-    PFZ_REQUIRE(!(matrix && gate), "pfz_dl_cand_argbest: the distance matrix needs every pair, so gate must be NULL with a matrix");
-    return run_k3<false, true>("pfz_dl_cand_argbest", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
-                               grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, 1, best_idx, best_score,
-                               best_dist, matrix, matrix_ld, gate, counter, stream, CandList{cand_idx, c, pos_of});
-}
-
-int pfz_dl_cand_topk(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
-                     int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
-                     const int32_t *sorig, int32_t n_to, int32_t metric, double score_cutoff, int32_t exclude_self, int64_t self_shift,
-                     const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t k, int32_t *top_idx, double *top_score,
-                     const double *gate, int32_t *counter, void *stream) {
-    PFZ_REQUIRE(metric == PFZ_METRIC_NORM_DL, "pfz_dl_cand_topk: metric %d unsupported (NORM_DL)", metric);
-    return run_k3<true, true>("pfz_dl_cand_topk", from_blob, from_offsets, n_from, from_ids, n_ids, n_words, sym_table, packed,
-                              grp_word_off, slen, sorig, n_to, metric, score_cutoff, exclude_self, self_shift, 1, k, top_idx, top_score,
-                              nullptr, nullptr, 0, gate, counter, stream, CandList{cand_idx, c, pos_of});
+    const bool dl = metric == PFZ_METRIC_DL || metric == PFZ_METRIC_NORM_DL;
+    if (k >= 1) {
+        PFZ_REQUIRE((metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER) || metric == PFZ_METRIC_NORM_OSA ||
+                    metric == PFZ_METRIC_NORM_DL,
+                    "pfz_lev_rows: top-k metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA, NORM_DL)", metric);
+        PFZ_REQUIRE(!part_dist && !matrix, "pfz_lev_rows: top-k has no distance output (part_dist and matrix must be NULL)");
+    } else {
+        PFZ_REQUIRE(part_dist, "pfz_lev_rows: arg-best needs part_dist");
+    }
+    PFZ_REQUIRE(!(jaro && matrix), "pfz_lev_rows: the distance matrix is not available for the Jaro metrics (matrix must be NULL)");
+    PFZ_REQUIRE(!gate || dl, "pfz_lev_rows: gate is for DL / NORM_DL only (gate must be NULL for metric %d)", metric);
+    PFZ_REQUIRE(!(matrix && gate), "pfz_lev_rows: the distance matrix needs every pair, so gate must be NULL with a matrix");
+    if (cand_idx)
+        PFZ_REQUIRE(n_splits == 1 && c >= 1 && pos_of, "pfz_lev_rows: candidate mode needs n_splits = 1, c >= 1 and pos_of "
+                    "(n_splits=%d, c=%d, pos_of %p)", n_splits, c, (const void *)pos_of);
+    else
+        PFZ_REQUIRE(n_splits >= 1, "pfz_lev_rows: n_splits < 1");
+    if (n_ids <= 0 || n_to < 0) return 0;
+    cudaStream_t st = as_stream(stream);
+    int sms = 0;
+    if (start_rows(counter, n_splits, st, &sms)) return 1;
+    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, metric, score_cutoff,
+                exclude_self, self_shift, ratio_min_ns_of(score_cutoff), n_splits, part_idx, part_score, part_dist, matrix, matrix_ld, n_from,
+                counter, k, CandList{cand_idx, c, pos_of}};
+    if (cand_idx) return k ? launch_class<true, true>(P, gate, n_words, sms, st) : launch_class<false, true>(P, gate, n_words, sms, st);
+    return k ? launch_class<true, false>(P, gate, n_words, sms, st) : launch_class<false, false>(P, gate, n_words, sms, st);
 }
 
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits, int32_t n_from,

@@ -1,4 +1,4 @@
-"""K3 host driver: all-pairs edit distance with per-row arg-best on the GPU (include/pfz.h, pfz_lev_*).
+"""K3 host driver: all-pairs edit distance with per-row arg-best on the GPU (include/pfz.h, pfz_lev_rows).
 
 Semantics restated from the reference's call sites (polyfuzz/models/_rapidfuzz.py:99-113,
 polyfuzz/models/_distance.py:89-102) and rapidfuzz's published definitions:
@@ -12,7 +12,7 @@ polyfuzz/models/_distance.py:89-102) and rapidfuzz's published definitions:
                 substring is edited twice, so osa("CA", "ABC") = 3 where unrestricted Damerau-Levenshtein gives 2)
     "norm_dl"   DamerauLevenshtein.normalized_similarity = 1 - dl/max(|a|,|b|)  in [0, 1]
     "dl"        raw unrestricted Damerau-Levenshtein distance (Lowrance-Wagner, unit costs: a swapped pair may be edited
-                again, so dl("CA", "ABC") = 2); computed by pfz_dl_*, gated by an OSA pass (DESIGN.md 4.10)
+                again, so dl("CA", "ABC") = 2); gated by an OSA pass (DESIGN.md 4.10)
 The Jaro metrics are computed on code points, from-string first (the reference calls scorer(from_string, to_string),
 polyfuzz/models/_distance.py:98); their best_dist is the number of matching characters, and they have no distance
 matrix (want_matrix=True raises ValueError).
@@ -45,7 +45,7 @@ MAX_LEN = 1024
 
 
 def _word_class(m):
-    """n_words argument of pfz_lev_argbest for a pattern of m code points."""
+    """n_words argument of pfz_lev_rows for a pattern of m code points."""
     if m <= 32:
         return 0
     for nw in (1, 2, 4, 8, 16):
@@ -202,72 +202,102 @@ def _word_classes(Q, T):
             yield d_table, nw, d_ids, n_ids
 
 
-def _k3_head(Q, T, cls, metric, score_cutoff, exclude_self, self_shift, n_splits):
-    """The leading arguments of pfz_lev_argbest, pfz_lev_topk, pfz_dl_argbest and pfz_dl_topk (from_blob .. n_splits)."""
-    d_table, nw, d_ids, n_ids = cls
-    return (_p(Q.d_blob), _p(Q.d_off), Q.n, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff), _p(T.slen),
-            _p(T.d_order), T.n, METRIC[metric], float(score_cutoff), int(bool(exclude_self)), int(self_shift), n_splits)
-
-
 def _gate_fill(metric, score_cutoff):
     """Gate of a row with fewer than k OSA candidates: the cutoff (norm_dl), or no bound (raw dl has no cutoff)."""
     return float(score_cutoff) if metric == "norm_dl" else float("-inf")
+
+
+def _empty(n_from, k):
+    """Rows with nothing to score: (idx, score, dist) [n_from] for the arg-best (k = 0), (idx, score) [n_from, k] for the k best;
+    every slot empty (-1, 0.0, -1)."""
+    dev = _dev()
+    shape = (n_from, k) if k else (n_from,)
+    out = (torch.full(shape, -1, dtype=torch.int32, device=dev), torch.zeros(shape, dtype=torch.float64, device=dev))
+    return out if k else out + (torch.full(shape, -1, dtype=torch.int32, device=dev),)
+
+
+def _rebase(idx, to_index_base):
+    """to_index_base added to the found indices (row-block shards); empty slots stay -1."""
+    return torch.where(idx >= 0, idx + int(to_index_base), idx) if to_index_base else idx
+
+
+def _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, k, n_splits=None, cand=None, matrix=None, dl_gate=True):
+    """Score Q against T with pfz_lev_rows, every alphabet batch and word class, and return the rows' results: k = 0 the
+    arg-best (idx, score, dist) [n_from], k >= 1 the k best (idx, score) [n_from, k].
+    cand None: all pairs over n_splits to-splits (None: default_splits), merged by pfz_lev_merge (the arg-best, even with one
+    split) or by pfz_topk_merge (the k best, more than one split).  cand (check_candidates): each row's own list, one split, no
+    merge.  matrix (arg-best, int32 [>= n_from, >= n_to] or None) receives the distances.
+    On all pairs a DL metric is gated per word class, unless dl_gate is False or a matrix is wanted: the same call with the
+    OSA metric of DL_GATE, merged, gives each row's k-th best OSA score (k = 1 for the arg-best; _gate_fill when it has fewer)."""
+    n_from = Q.n
+    if n_from == 0 or T.n == 0 or (cand is not None and cand.shape[1] == 0):
+        return _empty(n_from, k)
+    dev = _dev()
+    if cand is not None:
+        n_splits = 1
+    elif n_splits is None:
+        n_splits = default_splits(n_from, T.n_grp)
+    n_splits = max(1, min(int(n_splits), T.n_grp))
+    shape = (n_splits, n_from, k) if k else (n_splits, n_from)
+    part = [torch.full(shape, -1, dtype=torch.int32, device=dev), torch.zeros(shape, dtype=torch.float64, device=dev)]
+    if not k:
+        part.append(torch.full(shape, -1, dtype=torch.int32, device=dev))
+    counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
+    src = (_p(cand), int(cand.shape[1]), _p(T.d_pos_of)) if cand is not None else (None, 0, None)
+
+    def rows(d_table, nw, d_ids, n_ids, m, mat, gate):
+        _lib.call("pfz_lev_rows", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
+                  _p(T.slen), _p(T.d_order), T.n, METRIC[m], float(score_cutoff), int(bool(exclude_self)), int(self_shift), n_splits, k,
+                  *src, _p(part[0]), _p(part[1]), _p(part[2] if not k else None), _p(mat), int(mat.stride(0)) if mat is not None else 0,
+                  _p(gate), _p(counter), _stream())
+
+    def merged():
+        if cand is not None:
+            return tuple(t[0] for t in part)
+        if not k:
+            return lev_merge(*part)
+        return (part[0][0], part[1][0]) if n_splits == 1 else topk_merge(part[0], part[1], k)
+
+    gated = metric in DL_GATE and cand is None and matrix is None and dl_gate
+    for cls in _word_classes(Q, T):
+        gate = None
+        if gated:
+            rows(*cls, DL_GATE[metric], None, None)
+            gi, gs = merged()[:2]
+            if k:
+                gi, gs = gi[:, k - 1], gs[:, k - 1]
+            gate = torch.where(gi >= 0, gs, _gate_fill(metric, score_cutoff)).contiguous()
+        rows(*cls, metric, matrix, gate)
+    return merged()
 
 
 def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, want_matrix=False,
                         n_splits=None, to_index_base=0, dl_gate=True):
     """Kernels only.  Returns (best_idx int32[n_from] (-1 = none; + to_index_base otherwise), best_score float64[n_from],
     best_dist int32[n_from] [, matrix int32[n_from, n_to]]) as device tensors.
-    dl / norm_dl: per word class an OSA arg-best pass and its split merge give each row's gate, then pfz_dl_argbest;
+    dl / norm_dl: per word class an OSA arg-best pass and its split merge give each row's gate, then the DL pass;
     dl_gate=False (for timing) skips the OSA pass, and a matrix is computed without it."""
     if want_matrix and metric in JARO_METRICS:
         raise ValueError(f"want_matrix=True: the {metric!r} metric has no integer distance matrix")
-    dev = _dev()
-    n_from, n_to = Q.n, T.n
-    best_idx = torch.full((max(n_from, 1),), -1, dtype=torch.int32, device=dev)
-    best_score = torch.zeros(max(n_from, 1), dtype=torch.float64, device=dev)
-    best_dist = torch.full((max(n_from, 1),), -1, dtype=torch.int32, device=dev)
-    matrix = torch.zeros((max(n_from, 1), max(n_to, 1)), dtype=torch.int32, device=dev) if want_matrix else None
-    if n_from == 0 or n_to == 0:
-        out = (best_idx[:n_from], best_score[:n_from], best_dist[:n_from])
-        return out + (matrix[:n_from, :n_to],) if want_matrix else out
-    if n_splits is None:
-        n_splits = default_splits(n_from, T.n_grp)
-    n_splits = max(1, min(int(n_splits), T.n_grp))
-    part_idx = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
-    part_score = torch.zeros((n_splits, n_from), dtype=torch.float64, device=dev)
-    part_dist = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
-    counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
-    mat = (_p(matrix), int(matrix.stride(0)) if matrix is not None else 0)
-    for cls in _word_classes(Q, T):
-        head = lambda m: _k3_head(Q, T, cls, m, score_cutoff, exclude_self, self_shift, n_splits)  # noqa: E731
-        if metric not in DL_GATE:
-            _lib.call("pfz_lev_argbest", *head(metric), _p(part_idx), _p(part_score), _p(part_dist), *mat, _p(counter), _stream())
-            continue
-        gate = None
-        if dl_gate and not want_matrix:
-            _lib.call("pfz_lev_argbest", *head(DL_GATE[metric]), _p(part_idx), _p(part_score), _p(part_dist), None, 0, _p(counter),
-                      _stream())
-            _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx),
-                      _p(best_score), _p(best_dist), _stream())
-            gate = torch.where(best_idx >= 0, best_score, _gate_fill(metric, score_cutoff))
-        _lib.call("pfz_dl_argbest", *head(metric), _p(part_idx), _p(part_score), _p(part_dist), *mat, _p(gate), _p(counter),
-                  _stream())
-    _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx), _p(best_score),
-              _p(best_dist), _stream())
-    if to_index_base:
-        best_idx = torch.where(best_idx >= 0, best_idx + int(to_index_base), best_idx)
-    out = (best_idx[:n_from], best_score[:n_from], best_dist[:n_from])
-    return out + (matrix[:n_from, :n_to],) if want_matrix else out
+    matrix = torch.zeros((max(Q.n, 1), max(T.n, 1)), dtype=torch.int32, device=_dev()) if want_matrix else None
+    bi, bs, bd = _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, 0, n_splits, matrix=matrix, dl_gate=dl_gate)
+    out = (_rebase(bi, to_index_base), bs, bd)
+    return out + (matrix[:Q.n, :T.n],) if want_matrix else out
+
+
+def _stage(from_list, to_list, kept, reuse):
+    """EditQueries of from_list and EditTargets of to_list, the latter taken from kept (KeptTargets) when reuse allows it."""
+    _dev()
+    Q = EditQueries(from_list)
+    T = kept.stage(("k3", 0), to_list, EditTargets, reuse) if kept is not None else EditTargets(to_list)
+    return Q, T
 
 
 def edit_argbest(from_list, to_list, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0,
                  want_matrix=False, n_splits=None, dl_gate=True, kept=None, reuse=False):
     """Host lists in, device tensors out (see edit_argbest_staged).  kept (KeptTargets): where the staged to-side is kept;
     reuse: take it from there when it was staged from an equal to_list."""
-    _dev()
-    Q = EditQueries(from_list)
-    T = kept.stage(("k3", 0), to_list, EditTargets, reuse) if kept is not None else EditTargets(to_list)
+    Q, T = _stage(from_list, to_list, kept, reuse)
     return edit_argbest_staged(Q, T, metric, score_cutoff, exclude_self, self_shift, want_matrix, n_splits, dl_gate=dl_gate)
 
 
@@ -284,48 +314,23 @@ def check_top_n(k):
 
 def edit_topk_staged(Q, T, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, to_index_base=0,
                      dl_gate=True):
-    """Kernels only: the k best to-strings per from-string (pfz_lev_topk, then pfz_topk_merge over the to-splits), with the
+    """Kernels only: the k best to-strings per from-string (pfz_lev_rows, then pfz_topk_merge over the to-splits), with the
     candidates and the key of edit_argbest_staged.  Returns device (idx int32[n_from, k] (-1 = empty slot; + to_index_base
     otherwise), score float64[n_from, k] (0.0 in empty slots)).
     norm_dl: per word class a norm_osa top-k pass and its split merge give each row's gate (its k-th best OSA score), then
-    pfz_dl_topk; dl_gate=False (for timing) skips the OSA pass."""
+    the DL pass; dl_gate=False (for timing) skips the OSA pass."""
     k = check_top_n(k)
     if metric not in TOPK_METRICS:
         raise ValueError(f"top-k is available for the metrics {TOPK_METRICS}, not {metric!r}")
-    dev = _dev()
-    n_from, n_to = Q.n, T.n
-    if n_from == 0 or n_to == 0:
-        return (torch.full((n_from, k), -1, dtype=torch.int32, device=dev), torch.zeros((n_from, k), dtype=torch.float64, device=dev))
-    if n_splits is None:
-        n_splits = default_splits(n_from, T.n_grp)
-    n_splits = max(1, min(int(n_splits), T.n_grp))
-    part_idx = torch.full((n_splits, n_from, k), -1, dtype=torch.int32, device=dev)
-    part_score = torch.zeros((n_splits, n_from, k), dtype=torch.float64, device=dev)
-    counter = torch.zeros(n_splits, dtype=torch.int32, device=dev)
-    for cls in _word_classes(Q, T):
-        head = lambda m: _k3_head(Q, T, cls, m, score_cutoff, exclude_self, self_shift, n_splits)  # noqa: E731
-        if metric not in DL_GATE:
-            _lib.call("pfz_lev_topk", *head(metric), k, _p(part_idx), _p(part_score), _p(counter), _stream())
-            continue
-        gate = None
-        if dl_gate:
-            _lib.call("pfz_lev_topk", *head(DL_GATE[metric]), k, _p(part_idx), _p(part_score), _p(counter), _stream())
-            gi, gs = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
-            gate = torch.where(gi[:, k - 1] >= 0, gs[:, k - 1], _gate_fill(metric, score_cutoff)).contiguous()
-        _lib.call("pfz_dl_topk", *head(metric), k, _p(part_idx), _p(part_score), _p(gate), _p(counter), _stream())
-    idx, score = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
-    if to_index_base:
-        idx = torch.where(idx >= 0, idx + int(to_index_base), idx)
-    return idx, score
+    idx, score = _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, k, n_splits, dl_gate=dl_gate)
+    return _rebase(idx, to_index_base), score
 
 
 def edit_topk(from_list, to_list, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, dl_gate=True,
               kept=None, reuse=False):
     """Host lists in, device tensors out (see edit_topk_staged); kept and reuse as in edit_argbest."""
     k = check_top_n(k)
-    _dev()
-    Q = EditQueries(from_list)
-    T = kept.stage(("k3", 0), to_list, EditTargets, reuse) if kept is not None else EditTargets(to_list)
+    Q, T = _stage(from_list, to_list, kept, reuse)
     return edit_topk_staged(Q, T, k, metric, score_cutoff, exclude_self, self_shift, n_splits, dl_gate=dl_gate)
 
 
@@ -357,7 +362,7 @@ def check_candidates(cand, n_from, n_to):
 
 
 def edit_cand_topk_staged(Q, T, cand, k, metric="ratio", score_cutoff=0.0, exclude_self=False, self_shift=0):
-    """Kernels only (pfz_lev_cand_* / pfz_dl_cand_*): per from-row the k best to-strings among its candidates cand[i]
+    """Kernels only (pfz_lev_rows in candidate mode): per from-row the k best to-strings among its candidates cand[i]
     (check_candidates), under the metrics, cutoffs, self-exclusion and key of edit_argbest_staged / edit_topk_staged.
     k = 1 returns what edit_argbest_staged returns (best_idx, best_score, best_dist), any metric; k > 1 returns
     (idx int32[n_from, k], score float64[n_from, k]) as edit_topk_staged, metrics TOPK_METRICS.  A row with no candidate that
@@ -367,35 +372,13 @@ def edit_cand_topk_staged(Q, T, cand, k, metric="ratio", score_cutoff=0.0, exclu
         raise ValueError(f"top-k is available for the metrics {TOPK_METRICS}, not {metric!r}")
     if metric not in METRIC:
         raise ValueError(f"unknown metric {metric!r}")
-    dev = _dev()
-    n_from, n_to = Q.n, T.n
-    cand = check_candidates(cand, n_from, n_to)
-    c = int(cand.shape[1])
-    shape = (max(n_from, 1),) if k == 1 else (max(n_from, 1), k)
-    idx = torch.full(shape, -1, dtype=torch.int32, device=dev)
-    score = torch.zeros(shape, dtype=torch.float64, device=dev)
-    dist = torch.full(shape, -1, dtype=torch.int32, device=dev) if k == 1 else None
-    if n_from and n_to and c:
-        counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        dl = metric in DL_GATE
-        for cls in _word_classes(Q, T):
-            head = _k3_head(Q, T, cls, metric, score_cutoff, exclude_self, self_shift, 1)[:-1] + (_p(cand), c, _p(T.d_pos_of))
-            gate = (None,) if dl else ()
-            if k == 1:
-                _lib.call("pfz_dl_cand_argbest" if dl else "pfz_lev_cand_argbest", *head, _p(idx), _p(score), _p(dist), None, 0, *gate,
-                          _p(counter), _stream())
-            else:
-                _lib.call("pfz_dl_cand_topk" if dl else "pfz_lev_cand_topk", *head, k, _p(idx), _p(score), *gate, _p(counter),
-                          _stream())
-    if k == 1:
-        return idx[:n_from], score[:n_from], dist[:n_from]
-    return idx[:n_from], score[:n_from]
+    cand = check_candidates(cand, Q.n, T.n)
+    # k = 1 takes the arg-best epilogue, which also gives the distance
+    return _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, 0 if k == 1 else k, cand=cand)
 
 
 def edit_cand_topk(from_list, to_list, cand, k, metric="ratio", score_cutoff=0.0, exclude_self=False, kept=None, reuse=False):
     """Host lists in, device tensors out (see edit_cand_topk_staged); kept and reuse as in edit_argbest."""
     k = check_top_n(k)
-    _dev()
-    Q = EditQueries(from_list)
-    T = kept.stage(("k3", 0), to_list, EditTargets, reuse) if kept is not None else EditTargets(to_list)
+    Q, T = _stage(from_list, to_list, kept, reuse)
     return edit_cand_topk_staged(Q, T, cand, k, metric, score_cutoff, exclude_self)

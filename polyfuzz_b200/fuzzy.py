@@ -1,6 +1,6 @@
 """K3b host driver: rapidfuzz's token / partial / weighted scorers (WRatio, partial_ratio, token_sort_ratio, token_set_ratio,
 token_ratio, partial_token_*_ratio, QRatio) over the |from| x |to| grid with a fused per-row arg-best on the GPU
-(include/pfz.h, pfz_fuzz_argbest; csrc/pfz_fuzz.cu).
+(include/pfz.h, pfz_fuzz_rows; csrc/pfz_fuzz.cu).
 
 Replaces the scorer loop of polyfuzz/models/_rapidfuzz.py:99-113 (process.extractOne with scorer=fuzz.WRatio, the
 reference's default, :48) and polyfuzz/models/_distance.py:89-102 for those scorers.  The host only packs each list into a
@@ -21,8 +21,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .editdist import (_alphabet_batches, _blob_to_dev, check_candidates, check_top_n, default_splits, group_word_offsets,
-                       inverse_order, symbol_table)
+from .editdist import (_alphabet_batches, _blob_to_dev, _empty, _rebase, check_candidates, check_top_n, default_splits,
+                       group_word_offsets, inverse_order, lev_merge, symbol_table)
 from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
@@ -123,9 +123,9 @@ def _call_ids(F, T, same):
 def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift, to_index_base, k, kept=None, reuse=False,
              cand=None):
     """Stage the from-list (and the to-list, unless `kept` -- an editdist.KeptTargets -- holds it already and `reuse` allows
-    it), join the two vocabularies, and enqueue K3b for every alphabet batch and word class: pfz_fuzz_argbest with part_*
-    [n_splits, n_from] when k is None, else pfz_fuzz_topk with part_* [n_splits, n_from, k].  cand (a checked candidate
-    array): pfz_fuzz_cand_argbest / pfz_fuzz_cand_topk with one split.  Returns (part_idx, part_score, n_splits, staged):
+    it), join the two vocabularies, and enqueue pfz_fuzz_rows for every alphabet batch and word class: the arg-best with part_*
+    [n_splits, n_from] when k is None, else the k best with part_* [n_splits, n_from, k].  cand (a checked candidate array):
+    each row's own list, one split.  Returns (part_idx, part_score, n_splits, staged):
     `staged` keeps the staged buffers alive until the caller has synchronised."""
     dev = _dev()
     n_from, n_to = len(from_list), len(to_list)
@@ -173,21 +173,33 @@ def _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, s
                 tens += [packs[v][0], packs[v][1], packs[v][2]]
             tens += [d_order, d_tok_blob, d_tok_off, part_idx, part_score, counter, None]
             arr = (ctypes.c_void_p * len(tens))(*[t.data_ptr() if t is not None else 0 for t in tens])
-            if cand is not None:
-                tail = (_p(cand), int(cand.shape[1]), _p(targets.d_pos_of))
-                if k is None:
-                    _lib.call("pfz_fuzz_cand_argbest", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer],
-                              float(score_cutoff), int(bool(exclude_self)), int(self_shift), *tail, _stream())
-                else:
-                    _lib.call("pfz_fuzz_cand_topk", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
-                              int(bool(exclude_self)), int(self_shift), *tail, int(k), _stream())
-            elif k is None:
-                _lib.call("pfz_fuzz_argbest", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
-                          int(bool(exclude_self)), int(self_shift), n_splits, _stream())
-            else:
-                _lib.call("pfz_fuzz_topk", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
-                          int(bool(exclude_self)), int(self_shift), n_splits, int(k), _stream())
+            src = (_p(cand), int(cand.shape[1]), _p(targets.d_pos_of)) if cand is not None else (None, 0, None)
+            _lib.call("pfz_fuzz_rows", arr, len(tens), n_from, len(ids), int(nw), n_to, SCORER[scorer], float(score_cutoff),
+                      int(bool(exclude_self)), int(self_shift), n_splits, int(k or 0), *src, _stream())
     return part_idx, part_score, n_splits, (F, targets, keep, d_tok_blob, d_tok_off)
+
+
+def _scores(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift, to_index_base, k, kept, reuse, cand=None):
+    """The rows' results of the public functions: (idx, score) [n_from] for the arg-best (k None), [n_from, k] for the k best.
+    _enqueue, then the split merge (pfz_lev_merge for the arg-best even with one split, pfz_topk_merge over more than one split,
+    none in candidate mode), the synchronise and to_index_base added to the found indices."""
+    if scorer not in SCORER:
+        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
+    n_from, n_to = len(from_list), len(to_list)
+    if cand is not None:
+        cand = check_candidates(cand, n_from, n_to)
+    if n_from == 0 or n_to == 0 or (cand is not None and cand.shape[1] == 0):
+        return _empty(n_from, k or 0)[:2]
+    part_idx, part_score, n_splits, staged = _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift,
+                                                      to_index_base, k, kept, reuse, cand)
+    if cand is not None or (k is not None and n_splits == 1):
+        idx, score = part_idx[0], part_score[0]
+    elif k is None:
+        idx, score, _ = lev_merge(part_idx, part_score, torch.full_like(part_idx, -1))
+    else:
+        idx, score = topk_merge(part_idx, part_score, k)
+    torch.cuda.current_stream().synchronize()                  # the staged host buffers above go out of scope with this call
+    return _rebase(idx, to_index_base), score
 
 
 def fuzz_argbest(from_list, to_list, scorer="WRatio", score_cutoff=0.0, exclude_self=False, n_splits=None, self_shift=0,
@@ -197,24 +209,7 @@ def fuzz_argbest(from_list, to_list, scorer="WRatio", score_cutoff=0.0, exclude_
     exclude_self skips to-row == from-row + self_shift; to_index_base is added to the returned indices (row-block shards).
     kept (editdist.KeptTargets): where the staged to-side is kept; reuse: take it from there when it was staged from an equal
     to_list."""
-    if scorer not in SCORER:
-        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
-    dev = _dev()
-    n_from, n_to = len(from_list), len(to_list)
-    best_idx = torch.full((max(n_from, 1),), -1, dtype=torch.int32, device=dev)
-    best_score = torch.zeros(max(n_from, 1), dtype=torch.float64, device=dev)
-    if n_from == 0 or n_to == 0:
-        return best_idx[:n_from], best_score[:n_from]
-    part_idx, part_score, n_splits, staged = _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift,
-                                                      to_index_base, None, kept, reuse)
-    part_dist = torch.full((n_splits, n_from), -1, dtype=torch.int32, device=dev)
-    best_dist = torch.empty(max(n_from, 1), dtype=torch.int32, device=dev)
-    _lib.call("pfz_lev_merge", _p(part_idx), _p(part_score), _p(part_dist), n_splits, n_from, _p(best_idx), _p(best_score), _p(best_dist),
-              _stream())
-    torch.cuda.current_stream().synchronize()                  # the staged host buffers above go out of scope with this call
-    if to_index_base:
-        best_idx = torch.where(best_idx >= 0, best_idx + int(to_index_base), best_idx)
-    return best_idx[:n_from], best_score[:n_from]
+    return _scores(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift, to_index_base, None, kept, reuse)
 
 
 def fuzz_topk(from_list, to_list, k, scorer="WRatio", score_cutoff=0.0, exclude_self=False, n_splits=None, self_shift=0,
@@ -223,19 +218,7 @@ def fuzz_topk(from_list, to_list, k, scorer="WRatio", score_cutoff=0.0, exclude_
     Returns device tensors (idx int32[n_from, k] (-1: empty slot), score float64[n_from, k] (0.0 in empty slots));
     exclude_self, self_shift, to_index_base, kept and reuse as in fuzz_argbest."""
     k = check_top_n(k)
-    if scorer not in SCORER:
-        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
-    dev = _dev()
-    n_from, n_to = len(from_list), len(to_list)
-    if n_from == 0 or n_to == 0:
-        return (torch.full((n_from, k), -1, dtype=torch.int32, device=dev), torch.zeros((n_from, k), dtype=torch.float64, device=dev))
-    part_idx, part_score, n_splits, staged = _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift,
-                                                      to_index_base, k, kept, reuse)
-    idx, score = (part_idx[0], part_score[0]) if n_splits == 1 else topk_merge(part_idx, part_score, k)
-    torch.cuda.current_stream().synchronize()                  # the staged host buffers above go out of scope with this call
-    if to_index_base:
-        idx = torch.where(idx >= 0, idx + int(to_index_base), idx)
-    return idx, score
+    return _scores(from_list, to_list, scorer, score_cutoff, exclude_self, n_splits, self_shift, to_index_base, k, kept, reuse)
 
 
 def fuzz_cand_topk(from_list, to_list, cand, k, scorer="WRatio", score_cutoff=0.0, exclude_self=False, kept=None, reuse=False):
@@ -244,15 +227,4 @@ def fuzz_cand_topk(from_list, to_list, cand, k, scorer="WRatio", score_cutoff=0.
     fuzz_argbest returns (best_idx int32[n_from], best_score float64[n_from]); k > 1 what fuzz_topk returns.  A row with no
     candidate that passes gets (-1, 0.0); exclude_self, kept and reuse as in fuzz_argbest."""
     k = check_top_n(k)
-    if scorer not in SCORER:
-        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: {sorted(SCORER)})")
-    dev = _dev()
-    n_from, n_to = len(from_list), len(to_list)
-    cand = check_candidates(cand, n_from, n_to)
-    if n_from == 0 or n_to == 0 or cand.shape[1] == 0:
-        shape = (n_from,) if k == 1 else (n_from, k)
-        return torch.full(shape, -1, dtype=torch.int32, device=dev), torch.zeros(shape, dtype=torch.float64, device=dev)
-    part_idx, part_score, _, staged = _enqueue(from_list, to_list, scorer, score_cutoff, exclude_self, 1, 0, 0, None if k == 1 else k,
-                                               kept, reuse, cand)
-    torch.cuda.current_stream().synchronize()                  # the staged host buffers above go out of scope with this call
-    return part_idx[0], part_score[0]
+    return _scores(from_list, to_list, scorer, score_cutoff, exclude_self, 1, 0, 0, None if k == 1 else k, kept, reuse, cand)

@@ -1,5 +1,5 @@
-"""GPU tests of candidate mode: K3 / K3b score each from-row against its own candidate list (pfz_lev_cand_*, pfz_dl_cand_*,
-pfz_fuzz_cand_*; editdist.edit_cand_topk_staged, fuzzy.fuzz_cand_topk) and RapidFuzz / EditDistance(candidates=TFIDF(...)).
+"""GPU tests of candidate mode: K3 / K3b score each from-row against its own candidate list (pfz_lev_rows and
+pfz_fuzz_rows with cand_idx; editdist.edit_cand_topk_staged, fuzzy.fuzz_cand_topk) and RapidFuzz / EditDistance(candidates=TFIDF(...)).
 
 The defining property: a row equals the all-pairs result of the same scorer against the to-strings of its candidate list,
 indices mapped back, scores bit for bit.  Checked three ways:
@@ -394,9 +394,9 @@ def test_cutoffs_at_achievable_scores(ed, fz):
                     _eq(_cand(ed, None, metric, frm, to, cand, k, c), orc.topk(cand, k))
 
 
-def test_matrix_and_gate_of_the_argbest_entry_points(ed):
-    """pfz_lev_cand_argbest / pfz_dl_cand_argbest with a matrix: the candidate pairs' cells hold their distances, the rest
-    is untouched; pfz_dl_cand_argbest with a gate (each row's best OSA score over its list) returns the ungated result."""
+def test_matrix_and_gate_of_lev_rows_in_candidate_mode(ed):
+    """pfz_lev_rows in candidate mode with k = 0 and a matrix: the candidate pairs' cells hold their distances, the rest is
+    untouched; with dl and a gate (each row's best OSA score over its list) it returns the ungated result."""
     import torch
     from polyfuzz_b200 import _lib
     from polyfuzz_b200.engine import _p, _stream
@@ -406,17 +406,21 @@ def test_matrix_and_gate_of_the_argbest_entry_points(ed):
     cand = _random_lists(rng, len(frm), len(to), 20)
     Q, T = ed.EditQueries(frm), ed.EditTargets(to)
     dc = _dev(cand)
-    for metric, name, D in (("lev", "pfz_lev_cand_argbest", onative.editdist_matrix(frm, to, "lev")),
-                            ("osa", "pfz_lev_cand_argbest", osa_oracle.osa_matrix(frm, to)),
-                            ("dl", "pfz_dl_cand_argbest", dl_oracle.dl_matrix(frm, to))):
+
+    def rows(metric, mat, gate):
         out = [torch.full((len(frm),), -1, dtype=torch.int32, device="cuda"), torch.zeros(len(frm), dtype=torch.float64, device="cuda"),
                torch.full((len(frm),), -1, dtype=torch.int32, device="cuda")]
-        mat = torch.full((len(frm), len(to)), -7, dtype=torch.int32, device="cuda")
         counter = torch.zeros(1, dtype=torch.int32, device="cuda")
-        for cls in ed._word_classes(Q, T):
-            head = ed._k3_head(Q, T, cls, metric, 0.0, False, 0, 1)[:-1] + (_p(dc), cand.shape[1], _p(T.d_pos_of))
-            _lib.call(name, *head, *[_p(t) for t in out], _p(mat), int(mat.stride(0)), *((None,) if metric == "dl" else ()),
-                      _p(counter), _stream())
+        for d_table, nw, d_ids, n_ids in ed._word_classes(Q, T):
+            _lib.call("pfz_lev_rows", _p(Q.d_blob), _p(Q.d_off), Q.n, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
+                      _p(T.slen), _p(T.d_order), T.n, ed.METRIC[metric], 0.0, 0, 0, 1, 0, _p(dc), cand.shape[1], _p(T.d_pos_of),
+                      *[_p(t) for t in out], _p(mat), int(mat.stride(0)) if mat is not None else 0, _p(gate), _p(counter), _stream())
+        return out
+
+    for metric, D in (("lev", onative.editdist_matrix(frm, to, "lev")), ("osa", osa_oracle.osa_matrix(frm, to)),
+                      ("dl", dl_oracle.dl_matrix(frm, to))):
+        mat = torch.full((len(frm), len(to)), -7, dtype=torch.int32, device="cuda")
+        out = rows(metric, mat, None)
         m = mat.cpu().numpy()
         exp = np.full_like(m, -7)
         for i in range(len(frm)):
@@ -429,12 +433,7 @@ def test_matrix_and_gate_of_the_argbest_entry_points(ed):
     # the gate: the best norm_osa score over each row's list bounds its best norm_dl score from below
     oi, os_, _ = ed.edit_cand_topk_staged(Q, T, dc, 1, "norm_osa", 0.0)
     gate = torch.where(oi >= 0, os_, 0.0).contiguous()
-    out = [torch.full((len(frm),), -1, dtype=torch.int32, device="cuda"), torch.zeros(len(frm), dtype=torch.float64, device="cuda"),
-           torch.full((len(frm),), -1, dtype=torch.int32, device="cuda")]
-    counter = torch.zeros(1, dtype=torch.int32, device="cuda")
-    for cls in ed._word_classes(Q, T):
-        head = ed._k3_head(Q, T, cls, "norm_dl", 0.0, False, 0, 1)[:-1] + (_p(dc), cand.shape[1], _p(T.d_pos_of))
-        _lib.call("pfz_dl_cand_argbest", *head, *[_p(t) for t in out], None, 0, _p(gate), _p(counter), _stream())
+    out = rows("norm_dl", None, gate)
     ref = ed.edit_cand_topk_staged(Q, T, dc, 1, "norm_dl", 0.0)
     for a, b in zip(out[:2], ref[:2]):
         np.testing.assert_array_equal(a.cpu().numpy(), b.cpu().numpy())

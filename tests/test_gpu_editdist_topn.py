@@ -1,4 +1,4 @@
-"""GPU tests of the top-k epilogue of K3 / K3b (pfz_lev_topk, pfz_fuzz_topk) and of RapidFuzz / EditDistance with top_n > 1.
+"""GPU tests of the top-k epilogue of K3 / K3b (pfz_lev_rows, pfz_fuzz_rows with k >= 1) and of RapidFuzz / EditDistance with top_n > 1.
 The oracle is a full score matrix sorted by the canonical key (score desc, to-index asc): ratio / norm_lev from the
 Wagner-Fischer distances of oracle.native with the kernel's IEEE expressions (numpy has no FMA, so they are exact), the
 K3b scorers from oracle/fuzz.py, Jaro from tests/jaro_oracle.py.  Indices and scores are compared with ==."""

@@ -1,4 +1,4 @@
-"""Developer tool: time K3b (pfz_fuzz_argbest) on long from-strings, per word class, for WRatio, partial_ratio and
+"""Developer tool: time K3b (pfz_fuzz_rows, arg-best) on long from-strings, per word class, for WRatio, partial_ratio and
 token_set_ratio.
 
     python tools/fuzz_long_time.py [--runs 10] [--warmup 1] [--n-from 16] [--n-self 128] [--json OUT]
@@ -6,7 +6,7 @@ token_set_ratio.
 Input: seeded long strings made of movie titles (the c3 fixture, or its synthetic stand-in) joined with spaces until they
 reach a length drawn in the class's range: 200..256 code points (4 words), 300..512 (8 words, one CTA per row) and
 513..1 000 (16 words).  Each class is scored against the IMDB list (--n-from rows x 80 852) and against itself (--n-self
-rows, self-match).  Kernel time: CUDA events recorded on the stream right before and after each pfz_fuzz_argbest call (the
+rows, self-match).  Kernel time: CUDA events recorded on the stream right before and after each pfz_fuzz_rows call (the
 host staging of the call runs before the first event, and a short device sleep queued ahead of it keeps the entry point's
 own host set-up out of the interval), summed over the call's launches; the median of --runs calls after
 --warmup is reported with pairs/s.  The card's name, power limit and SM clocks are read in the same run."""
@@ -63,10 +63,10 @@ def main():
     pool = titles["Netflix"] + imdb
     kernel_ms = []
 
-    class Timed:                                            # events around the pfz_fuzz_* launches of one call
+    class Timed:                                            # events around the pfz_fuzz_rows launches of one call
         @staticmethod
         def call(name, *a):
-            if not name.startswith("pfz_fuzz_"):
+            if name != "pfz_fuzz_rows":
                 return _lib.call(name, *a)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             torch.cuda._sleep(4_000_000)                    # ~2 ms of device work ahead of e0: the call's host set-up
