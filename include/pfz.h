@@ -285,6 +285,25 @@ int pfz_lev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits,
                   int32_t n_from, int32_t *best_idx, double *best_score, int32_t *best_dist, void *stream);
 
+/* Weighted Levenshtein, rapidfuzz's Levenshtein.normalized_similarity(from, to, weights=(w_insert, w_delete, w_substitute)), with
+ * pfz_lev_rows's arguments and rules except metric, matrix and gate (csrc/pfz_lev.cu, wlev_kernel; DESIGN.md 4.17).
+ *   D: the Wagner-Fischer minimum on code points, w_insert per character of the to-string inserted, w_delete per character of the
+ *      from-string deleted, w_substitute per substitution, a match free.  M: min(m*wd + n*wi, n*ws + (m-n)*wd) when m >= n, else
+ *      min(m*wd + n*wi, m*ws + (n-m)*wi) (m, n: from / to lengths).  Score 1 - D/M in float64 (1 when M = 0); a candidate needs
+ *      score >= score_cutoff; key, exclusion, epilogues (k), sources (cand_idx) and merges as pfz_lev_rows.
+ *   weights: each in [0, PFZ_WLEV_MAX_WEIGHT].  w_insert = w_delete >= 1 with w_substitute >= 2*w_insert runs the Indel form
+ *      (score 1 - indel/(m+n), the same double); any other triple bounds D by the unit Levenshtein distance and runs an exact DP
+ *      on the pairs the bounds do not settle.
+ *   part_dist (arg-best only, required): D of the best pair, saturated at INT32_MAX.
+ * n_ids <= 0 (or n_to < 0) returns 0 without launching anything.                                                          */
+#define PFZ_WLEV_MAX_WEIGHT 65535
+int pfz_wlev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                  int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off,
+                  const int32_t *slen, const int32_t *sorig, int32_t n_to, int32_t w_insert, int32_t w_delete,
+                  int32_t w_substitute, double score_cutoff, int32_t exclude_self, int64_t self_shift, int32_t n_splits,
+                  int32_t k, const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *part_idx,
+                  double *part_score, int32_t *part_dist, int32_t *counter, void *stream);
+
 /* K3b  rapidfuzz's token / partial / weighted scorers with a fused per-row epilogue (csrc/pfz_fuzz.cu).
  * Replaces: process.extractOne / process.extract(query, to_list, scorer=fuzz.WRatio | partial_ratio | token_*_ratio | ...,
  *           score_cutoff, limit=k) at polyfuzz/models/_rapidfuzz.py:48,106-108 and the scorer loop of polyfuzz/models/_distance.py:98.

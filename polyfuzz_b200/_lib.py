@@ -43,6 +43,8 @@ _PROTOS = {
     "pfz_lev_rows": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_f64, c_i32, c_i64, c_i32,
                      c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp],
     "pfz_lev_merge": [c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp],
+    "pfz_wlev_rows": [c_vp, c_vp, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64,
+                      c_i32, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_fuzz_rows": [c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f64, c_i32, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, c_vp],
     "pfz_tok_side": [c_vp, c_vp, c_i32, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],
     "pfz_tok_union": [c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp],

@@ -16,8 +16,9 @@
 // NW 64-bit blocks with horizontal carries (Hyyro 2003).  Work is integer-ALU bound (SURVEY.md 8d).
 //
 // Shared by the kernels here: the row driver of pfz_common.cuh (split_groups, claim_row, build_peq, WarpArgBest / WarpTopK,
-// launch_rows), LevColumn (the Levenshtein / OSA column step of lev_kernel and dl_kernel), for_each_text_symbol (the text
-// loop), dispatch_words (n_words -> <W, NW>) and launch_class (the metric -> kernel choice of pfz_lev_rows).
+// launch_rows), LevColumn (the Levenshtein / OSA column step of lev_kernel, dl_kernel and wlev_kernel), for_each_text_symbol (the text
+// loop), dispatch_words (n_words -> <W, NW>), launch_class (the metric -> kernel choice of pfz_lev_rows) and launch_wlev
+// (pfz_wlev_rows).
 #include "pfz_common.cuh"
 #include <math_constants.h>
 #include <cmath>
@@ -192,6 +193,41 @@ struct LevColumn {
         return hin;
     }
 };
+
+// Length of the longest common subsequence of the pattern (match masks peq, m symbols) and the lane's text (n symbols in the
+// packed column src): Hyyro 2004's bit-parallel recurrence, one column per text symbol.  wlev_kernel's Indel form calls it;
+// lev_kernel keeps its own inline copy of the same loop, because calling this helper there reschedules its SASS.
+template <typename W, int NW>
+__device__ __forceinline__ int lcs_length(const W *peq, const uint32_t *src, int n, int m, int last_blk, int last_bit) {
+    constexpr int B = WordOps<W>::BITS;
+    W S[NW];
+#pragma unroll
+    for (int b = 0; b < NW; ++b) S[b] = ~(W)0;
+    for_each_text_symbol(src, n, [&](int s) {
+        unsigned carry = 0;
+#pragma unroll
+        for (int b = 0; b < NW; ++b) {
+            if (b <= last_blk) {
+                const W Eq = peq[s * NW + b];
+                const W x = S[b], u = x & Eq;
+                // S' = (S + (S & Eq)) | (S - (S & Eq)); u is a subset of x, so x - u = x & ~Eq (no borrow);
+                // the addition carries across blocks
+                const W sum = x + u; unsigned c1 = sum < x; const W sum2 = sum + carry; c1 |= (sum2 < sum); carry = c1;
+                S[b] = sum2 | (x & ~Eq);
+            }
+        }
+    });
+    int lcs = 0;
+#pragma unroll
+    for (int b = 0; b < NW; ++b) {
+        if (m > 0 && b <= last_blk) {
+            W z = ~S[b];
+            if (b == last_blk && last_bit != B - 1) z &= (((W)1 << (last_bit + 1)) - 1);
+            lcs += WordOps<W>::pop(z);
+        }
+    }
+    return lcs;
+}
 
 // One warp scores pattern `pat` against every to-string of its split.  LCS = false: Levenshtein, or with OSA = true optimal
 // string alignment (LevColumn); LCS = true: longest common subsequence (Hyyro 2004) -> Indel = la + lb - 2*LCS.
@@ -599,6 +635,187 @@ __global__ void __launch_bounds__(WARPS * 32, 1) dl_kernel(const LevParams P, co
     }
 }
 
+// ---- weighted Levenshtein (DESIGN.md 4.17) -----------------------------------------------------------------------------------
+// rapidfuzz's Levenshtein with weights = (insertion wi, deletion wd, substitution ws), s1 = the from-string (pattern), s2 = the
+// to-string (text): D = the Wagner-Fischer minimum (a match takes the diagonal for free), M = the weighted maximum (wlev_max), score
+// 1 - D / M (1 when M = 0).  INDEL (wi = wd >= 1, ws >= 2 wi): D = wi * indel, M = wi * (m + n), and each pair is exact from the LCS
+// recurrence.  Otherwise the unit Levenshtein distance L of the pair (LevColumn) brackets D (wlev_bounds); equal bounds give the
+// score, a pair whose score bound 1 - LB / M is below the running k-th score or the cutoff is dropped, and the rest are queued for
+// the exact DP (wlev_dp), 32 lanes abreast, as in dl_kernel.
+struct WlevWeights { int wi, wd, ws; };
+
+__device__ __forceinline__ int64_t wlev_max(const WlevWeights &w, int m, int n) {
+    const int64_t del_ins = (int64_t)m * w.wd + (int64_t)n * w.wi;
+    return min(del_ins, m >= n ? (int64_t)n * w.ws + (int64_t)(m - n) * w.wd : (int64_t)m * w.ws + (int64_t)(n - m) * w.wi);
+}
+
+__device__ __forceinline__ double wlev_score(int64_t d, int64_t M) { return M ? 1.0 - (double)d / (double)M : 1.0; }
+
+// LB <= D <= UB from the unit distance L (DESIGN.md 4.17 proves both): R = L - |m - n|, w_len the weight of the surplus side,
+// s = min(ws, wi + wd); LB = |m - n| w_len + ceil(R min(ws, (wi + wd) / 2)),
+// UB = min(M, |m - n| w_len + max(R s, floor(R / 2) (wi + wd) + (R mod 2) s)).
+struct WlevBounds { int64_t M, lb, ub; };
+__device__ __forceinline__ WlevBounds wlev_bounds(const WlevWeights &w, int L, int m, int n) {
+    const int64_t dlen = abs(m - n), R = L - dlen, len_cost = dlen * (m >= n ? w.wd : w.wi);
+    const int64_t pair = (int64_t)w.wi + w.wd, s = min((int64_t)w.ws, pair);
+    const int64_t M = wlev_max(w, m, n);
+    const int64_t lb = len_cost + (2 * (int64_t)w.ws <= pair ? R * w.ws : (R * pair + 1) / 2);
+    const int64_t ub = min(M, len_cost + max(R * s, R / 2 * pair + (R & 1) * s));
+    return {M, lb, ub};
+}
+
+// Exact weighted Levenshtein of pat[1..m] against the lane's text (n symbols in the packed column src), streamed column by column
+// over the text with O(m) state: E[r * 32] = d[r][j] - j * wi.  d[r][j] >= (j - r) wi (at least j - r insertions) and
+// d[r][j] <= d[0][j] + r wd, so E lies in [-r wi, r wd]: int32 at the weight cap for every pattern length and any text length.
+// Pattern symbols are >= 1 (every from-string code point is in the symbol table), so text-only symbol 0 matches nothing.
+__device__ __forceinline__ int64_t wlev_dp(const uint8_t *__restrict__ pat, int m, const uint32_t *__restrict__ src, int n,
+                                           const WlevWeights &w, int32_t *E) {
+    for (int r = 1; r <= m; ++r) E[r * 32] = r * w.wd;
+    const int sub = w.ws - w.wi;
+    int last = m * w.wd;
+    uint32_t word = 0;
+    for (int j = 0; j < n; ++j) {
+        if ((j & 3) == 0) word = src[(size_t)(j >> 2) * 32];
+        const int bj = (word >> (8 * (j & 3))) & 0xff;
+        int diag = 0, up = 0;                                   // E[0] = 0 in every column
+        for (int i = 1; i <= m; ++i) {
+            const int left = E[i * 32];
+            const int d = pat[i] == bj ? diag - w.wi : min(min(up + w.wd, left), diag + sub);
+            E[i * 32] = d;
+            diag = left; up = d;
+        }
+        last = up;
+    }
+    return (int64_t)last + (int64_t)n * w.wi;
+}
+
+template <typename W, int NW>
+struct WlevLayout {                     // one warp's shared memory (INDEL: the match masks only)
+    static constexpr int MAXM = WordOps<W>::BITS * NW;
+    static constexpr size_t PEQ = (size_t)256 * NW * sizeof(W);
+    static constexpr size_t QUEUE = 32 * (sizeof(double) + sizeof(int32_t));          // bound score, sorted to-position
+    static constexpr size_t STATE = (size_t)(MAXM + 1) * 32 * sizeof(int32_t);        // E: [row][lane]
+    static constexpr size_t PAT = (MAXM + 1 + 15) / 16 * 16;                          // pattern symbols, 1-based
+    static constexpr size_t PER_WARP = PEQ + QUEUE + STATE + PAT;
+    static_assert(PER_WARP % 16 == 0 && PER_WARP <= 227 * 1024, "weighted Levenshtein state does not fit one warp's shared memory");
+};
+
+template <typename W, int NW, int WARPS, bool TOPK, bool CAND, bool INDEL>
+__global__ void __launch_bounds__(WARPS * 32, 1) wlev_kernel(const LevParams P, const WlevWeights wt) {
+    constexpr int B = WordOps<W>::BITS;
+    using Lay = WlevLayout<W, NW>;
+    extern __shared__ __align__(16) unsigned char dyn[];
+    const int lane = lane_id();
+    unsigned char *base = dyn + (size_t)(threadIdx.x >> 5) * (INDEL ? Lay::PEQ : Lay::PER_WARP);
+    W *peq = reinterpret_cast<W *>(base);                                    // peq[sym * NW + block]
+    double *q_ub = reinterpret_cast<double *>(base + Lay::PEQ);
+    int32_t *q_pos = reinterpret_cast<int32_t *>(base + Lay::PEQ + 32 * sizeof(double));
+    int32_t *sE = reinterpret_cast<int32_t *>(base + Lay::PEQ + Lay::QUEUE) + lane;
+    uint8_t *pat = base + Lay::PEQ + Lay::QUEUE + Lay::STATE;
+    const double NEG_INF = -CUDART_INF;
+
+    for (;;) {
+        const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
+        if (i < 0) break;
+        const GroupRange gr = to_steps<CAND>(P.n_to, P.n_splits, P.cand);
+        const int64_t fb = P.from_off[i];
+        const int m = (int)(P.from_off[i + 1] - fb);
+        build_peq<W, NW>(peq, P.from_blob + fb, m, P.sym_table, INDEL ? nullptr : pat);
+        const int last_bit = (m - 1) & (B - 1);
+        const int last_blk = m > 0 ? (m - 1) / B : 0;
+
+        WarpArgBest<> best;
+        WarpTopK top;
+        if constexpr (TOPK) top.init(P.k); else best.init();
+        double kth = NEG_INF;                                               // warp-uniform running k-th exact score (not INDEL)
+        int qn = 0;                                                         // warp-uniform queue fill
+
+        auto offer = [&](bool have, int64_t d, int64_t M, int orig) {
+            double sc = 0.0; int cj = -1;
+            if (have) {
+                sc = wlev_score(d, M);
+                if (sc >= P.cutoff) cj = orig;
+            }
+            if constexpr (TOPK) {
+                top.offer(sc, cj);
+                if constexpr (!INDEL) {
+                    const double ts = shfl_d(top.s, P.k - 1);
+                    kth = __shfl_sync(FULL, top.j, P.k - 1) >= 0 ? ts : NEG_INF;
+                }
+            } else {
+                best.offer(sc, cj, (int)min(d, (int64_t)INT32_MAX));          // the distance, saturated
+                if constexpr (!INDEL) {
+                    double v = best.j >= 0 ? best.s : NEG_INF;
+#pragma unroll
+                    for (int o = 16; o; o >>= 1) v = fmax(v, shfl_d(v, lane ^ o));
+                    kth = v;
+                }
+            }
+        };
+        // all lanes: lane r < cnt takes queue entry r, re-tests its bound against the threshold (which may have risen since it
+        // was queued) and runs the DP
+        auto flush = [&](int cnt) {
+            const bool act = lane < cnt;
+            const int p = act ? q_pos[lane] : 0;
+            const int n = act ? P.slen[p] : 0;
+            const int orig = act ? P.sorig[p] : -1;
+            const bool run = act && !(q_ub[lane] < kth);
+            int64_t d = 0;
+            if (run) d = wlev_dp(pat, m, P.packed + P.grp_word_off[p >> 5] + (p & 31), n, wt, sE);
+            offer(run, d, wlev_max(wt, m, n), orig);
+        };
+
+        for (int g = gr.lo; g < gr.hi; ++g) {
+            const int p = to_pos<CAND>(g, i, P.cand);
+            const bool have = to_have<CAND>(p, P.n_to);
+            const int n = have ? P.slen[p] : 0;
+            const int orig = have ? P.sorig[p] : -1;
+            const uint32_t *src = to_column<CAND>(P.packed, P.grp_word_off, g, p);
+            WlevBounds bd;
+            if constexpr (INDEL) {
+                const int64_t indel = m + n - 2 * lcs_length<W, NW>(peq, src, n, m, last_blk, last_bit);
+                bd.M = (int64_t)wt.wi * (m + n); bd.lb = bd.ub = (int64_t)wt.wi * indel;
+            } else {
+                LevColumn<W, NW, false> col;
+                col.init();
+                int score_m = m;
+                for_each_text_symbol(src, n, [&](int s) { score_m += col.step(peq + s * NW, last_blk, last_bit); });
+                bd = wlev_bounds(wt, m > 0 ? score_m : n, m, n);
+            }
+            const bool excl = P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift;
+            const double ubs = wlev_score(bd.lb, bd.M);
+            bool direct = false, queued = false;
+            if (have && !excl && !(ubs < kth) && ubs >= P.cutoff) {
+                if (bd.lb == bd.ub) direct = true; else queued = true;
+            }
+            if (__any_sync(FULL, direct)) offer(direct, bd.lb, bd.M, orig);
+            if constexpr (!INDEL) {
+                const unsigned need = __ballot_sync(FULL, queued);
+                if (need) {
+                    const int pos = qn + __popc(need & ((1u << lane) - 1u));
+                    if (queued && pos < 32) { q_pos[pos] = p; q_ub[pos] = ubs; }
+                    int tot = qn + __popc(need);
+                    if (tot >= 32) {
+                        __syncwarp();
+                        flush(32);
+                        __syncwarp();
+                        if (queued && pos >= 32) { q_pos[pos - 32] = p; q_ub[pos - 32] = ubs; }
+                        tot -= 32;
+                    }
+                    qn = tot;
+                    __syncwarp();
+                }
+            }
+        }
+        if constexpr (!INDEL) {
+            if (qn > 0) flush(qn);
+        }
+
+        store_row<TOPK>(P, i, top, best);
+        __syncwarp();
+    }
+}
+
 template <typename W, int NW> struct WordClass { using Word = W; static constexpr int N = NW; };
 
 // n_words (0: one 32-bit word; 1, 2, 4, 8, 16 64-bit words) -> f(WordClass<W, NW>())
@@ -642,6 +859,25 @@ static int launch_class(const LevParams &P, const double *gate, int n_words, int
         if (mt == PFZ_METRIC_INDEL || mt == PFZ_METRIC_RATIO)
             return launch_rows(lev_kernel<W, NW, true, WARPS, TOPK, false, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
         return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK, false, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+    });
+}
+
+// word class -> wlev_kernel instantiation.  INDEL needs the match masks only (4 warps, as lev_kernel); the gated DP adds the queue,
+// the DP column and the pattern (WlevLayout): 5.5 KB per warp at 32 symbols, ..., 161.5 KB at 1 024 -- 4 warps per CTA up to 256
+// symbols, 2 at 512, 1 at 1 024.
+template <bool TOPK, bool CAND>
+static int launch_wlev(const LevParams &P, const WlevWeights &wt, bool indel, int n_words, int sms, cudaStream_t st) {
+    return dispatch_words(n_words, [&](auto c) {
+        using W = typename decltype(c)::Word;
+        constexpr int NW = decltype(c)::N;
+        if (indel) {
+            constexpr int WARPS = 4;
+            return launch_rows(wlev_kernel<W, NW, WARPS, TOPK, CAND, true>, WARPS, WARPS * WlevLayout<W, NW>::PEQ, P.n_ids, P.n_splits,
+                               sms, st, P, wt);
+        }
+        constexpr size_t PER_WARP = WlevLayout<W, NW>::PER_WARP;
+        constexpr int WARPS = warps_within(PER_WARP, 227 * 1024);
+        return launch_rows(wlev_kernel<W, NW, WARPS, TOPK, CAND, false>, WARPS, WARPS * PER_WARP, P.n_ids, P.n_splits, sms, st, P, wt);
     });
 }
 
@@ -700,6 +936,41 @@ int pfz_lev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
                 counter, k, CandList{cand_idx, c, pos_of}};
     if (cand_idx) return k ? launch_class<true, true>(P, gate, n_words, sms, st) : launch_class<false, true>(P, gate, n_words, sms, st);
     return k ? launch_class<true, false>(P, gate, n_words, sms, st) : launch_class<false, false>(P, gate, n_words, sms, st);
+}
+
+// The rules of pfz_lev_rows that apply (epilogue, source, part_dist) and the weight range are checked first, before any CUDA call;
+// then the weights pick INDEL (wi = wd >= 1, ws >= 2 wi) or the gated DP, and the <TOPK, CAND> instantiation runs.
+int pfz_wlev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
+                  int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off, const int32_t *slen,
+                  const int32_t *sorig, int32_t n_to, int32_t w_insert, int32_t w_delete, int32_t w_substitute, double score_cutoff,
+                  int32_t exclude_self, int64_t self_shift, int32_t n_splits, int32_t k, const int32_t *cand_idx, int32_t c,
+                  const int32_t *pos_of, int32_t *part_idx, double *part_score, int32_t *part_dist, int32_t *counter, void *stream) {
+    PFZ_REQUIRE(w_insert >= 0 && w_insert <= PFZ_WLEV_MAX_WEIGHT && w_delete >= 0 && w_delete <= PFZ_WLEV_MAX_WEIGHT &&
+                w_substitute >= 0 && w_substitute <= PFZ_WLEV_MAX_WEIGHT,
+                "pfz_wlev_rows: weights (%d, %d, %d) outside [0, %d]", w_insert, w_delete, w_substitute, PFZ_WLEV_MAX_WEIGHT);
+    PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
+                "pfz_wlev_rows: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
+    PFZ_REQUIRE(k >= 0 && k <= 32, "pfz_wlev_rows: k=%d unsupported (0 = arg-best, 1..32 = top-k)", k);
+    if (k >= 1)
+        PFZ_REQUIRE(!part_dist, "pfz_wlev_rows: top-k has no distance output (part_dist must be NULL)");
+    else
+        PFZ_REQUIRE(part_dist, "pfz_wlev_rows: arg-best needs part_dist");
+    if (cand_idx)
+        PFZ_REQUIRE(n_splits == 1 && c >= 1 && pos_of, "pfz_wlev_rows: candidate mode needs n_splits = 1, c >= 1 and pos_of "
+                    "(n_splits=%d, c=%d, pos_of %p)", n_splits, c, (const void *)pos_of);
+    else
+        PFZ_REQUIRE(n_splits >= 1, "pfz_wlev_rows: n_splits < 1");
+    if (n_ids <= 0 || n_to < 0) return 0;
+    cudaStream_t st = as_stream(stream);
+    int sms = 0;
+    if (start_rows(counter, n_splits, st, &sms)) return 1;
+    LevParams P{from_blob, from_offsets, from_ids, n_ids, sym_table, packed, grp_word_off, slen, sorig, n_to, PFZ_METRIC_NORM_LEV,
+                score_cutoff, exclude_self, self_shift, 0.0, n_splits, part_idx, part_score, part_dist, nullptr, 0, n_from, counter, k,
+                CandList{cand_idx, c, pos_of}};
+    const WlevWeights wt{w_insert, w_delete, w_substitute};
+    const bool indel = w_insert == w_delete && w_insert >= 1 && w_substitute >= 2 * w_insert;
+    if (cand_idx) return k ? launch_wlev<true, true>(P, wt, indel, n_words, sms, st) : launch_wlev<false, true>(P, wt, indel, n_words, sms, st);
+    return k ? launch_wlev<true, false>(P, wt, indel, n_words, sms, st) : launch_wlev<false, false>(P, wt, indel, n_words, sms, st);
 }
 
 int pfz_lev_merge(const int32_t *part_idx, const double *part_score, const int32_t *part_dist, int32_t n_splits, int32_t n_from,

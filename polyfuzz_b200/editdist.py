@@ -27,6 +27,11 @@ matcher's last staged to-side, which a `re_train=False` call with an equal to-li
 Candidate mode (`edit_cand_topk_staged`, DESIGN.md 4.16): each from-row scores only the to-indices of its row of a device
 int32 [n_from, c] candidate array (-1 = empty slot, distinct per row; TF-IDF's top-n), with the same kernels, scores, cutoffs
 and key, so a row equals the all-pairs result against the to-strings of its list.
+
+Weighted Levenshtein (`edit_wlev_argbest` / `edit_wlev_topk` / `edit_wlev_cand_topk` and their staged forms, pfz_wlev_rows,
+DESIGN.md 4.17): rapidfuzz's Levenshtein.normalized_similarity(from, to, weights=(insertion, deletion, substitution)) = 1 - D/M
+with norm_lev's key and cutoff, weights in [0, WLEV_MAX_WEIGHT].  Uniform weights (w, w, w) take the norm_lev path (the same
+scores); it is not a METRIC (no raw distance, no matrix).  It uses the same EditQueries / EditTargets / KeptTargets.
 """
 import numpy as np
 import torch
@@ -221,14 +226,16 @@ def _rebase(idx, to_index_base):
     return torch.where(idx >= 0, idx + int(to_index_base), idx) if to_index_base else idx
 
 
-def _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, k, n_splits=None, cand=None, matrix=None, dl_gate=True):
+def _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, k, n_splits=None, cand=None, matrix=None, dl_gate=True,
+               weights=None):
     """Score Q against T with pfz_lev_rows, every alphabet batch and word class, and return the rows' results: k = 0 the
     arg-best (idx, score, dist) [n_from], k >= 1 the k best (idx, score) [n_from, k].
     cand None: all pairs over n_splits to-splits (None: default_splits), merged by pfz_lev_merge (the arg-best, even with one
     split) or by pfz_topk_merge (the k best, more than one split).  cand (check_candidates): each row's own list, one split, no
     merge.  matrix (arg-best, int32 [>= n_from, >= n_to] or None) receives the distances.
     On all pairs a DL metric is gated per word class, unless dl_gate is False or a matrix is wanted: the same call with the
-    OSA metric of DL_GATE, merged, gives each row's k-th best OSA score (k = 1 for the arg-best; _gate_fill when it has fewer)."""
+    OSA metric of DL_GATE, merged, gives each row's k-th best OSA score (k = 1 for the arg-best; _gate_fill when it has fewer).
+    weights (check_weights, not None): weighted Levenshtein by pfz_wlev_rows instead; metric, matrix and dl_gate are unused."""
     n_from = Q.n
     if n_from == 0 or T.n == 0 or (cand is not None and cand.shape[1] == 0):
         return _empty(n_from, k)
@@ -246,6 +253,11 @@ def _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, k, n_splits
     src = (_p(cand), int(cand.shape[1]), _p(T.d_pos_of)) if cand is not None else (None, 0, None)
 
     def rows(d_table, nw, d_ids, n_ids, m, mat, gate):
+        if weights is not None:
+            _lib.call("pfz_wlev_rows", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
+                      _p(T.slen), _p(T.d_order), T.n, *weights, float(score_cutoff), int(bool(exclude_self)), int(self_shift), n_splits,
+                      k, *src, _p(part[0]), _p(part[1]), _p(part[2] if not k else None), _p(counter), _stream())
+            return
         _lib.call("pfz_lev_rows", _p(Q.d_blob), _p(Q.d_off), n_from, _p(d_ids), n_ids, nw, _p(d_table), _p(T.packed), _p(T.d_goff),
                   _p(T.slen), _p(T.d_order), T.n, METRIC[m], float(score_cutoff), int(bool(exclude_self)), int(self_shift), n_splits, k,
                   *src, _p(part[0]), _p(part[1]), _p(part[2] if not k else None), _p(mat), int(mat.stride(0)) if mat is not None else 0,
@@ -382,3 +394,98 @@ def edit_cand_topk(from_list, to_list, cand, k, metric="ratio", score_cutoff=0.0
     k = check_top_n(k)
     Q, T = _stage(from_list, to_list, kept, reuse)
     return edit_cand_topk_staged(Q, T, cand, k, metric, score_cutoff, exclude_self)
+
+
+# ---- weighted Levenshtein (DESIGN.md 4.17) ------------------------------------------------------------------------------------
+WLEV_MAX_WEIGHT = 65535                 # PFZ_WLEV_MAX_WEIGHT
+
+
+def check_weights(weights):
+    """rapidfuzz's Levenshtein `weights` = (insertion, deletion, substitution): None (unit costs) or a tuple / list of three ints
+    (Python or numpy integers, not bool), each in [0, WLEV_MAX_WEIGHT].  Returns None or a tuple of Python ints; anything else
+    raises ValueError."""
+    if weights is None:
+        return None
+    if (not isinstance(weights, (tuple, list)) or len(weights) != 3
+            or not all(isinstance(w, (int, np.integer)) and not isinstance(w, bool) and 0 <= w <= WLEV_MAX_WEIGHT for w in weights)):
+        raise ValueError(f"weights must be None or three ints (insertion, deletion, substitution) in [0, {WLEV_MAX_WEIGHT}], "
+                         f"got {weights!r}")
+    return tuple(int(w) for w in weights)
+
+
+def uniform_weight(weights):
+    """w for weights (w, w, w) with w >= 1, and 1 for None: D = w * lev and M = w * max(|a|, |b|), so the scores are norm_lev's
+    bit for bit.  0 for every other triple."""
+    if weights is None:
+        return 1
+    wi, wd, ws = weights
+    return wi if wi == wd == ws and wi >= 1 else 0
+
+
+def _wlev_rows(Q, T, weights, score_cutoff, exclude_self, self_shift, k, n_splits=None, cand=None):
+    """_edit_rows for weighted Levenshtein: uniform weights take the norm_lev path (its arg-best distances times w, saturated at
+    2^31 - 1 as pfz_wlev_rows saturates D), any other triple pfz_wlev_rows."""
+    weights = check_weights(weights)
+    w = uniform_weight(weights)
+    if not w:
+        return _edit_rows(Q, T, None, score_cutoff, exclude_self, self_shift, k, n_splits, cand, weights=weights)
+    out = _edit_rows(Q, T, "norm_lev", score_cutoff, exclude_self, self_shift, k, n_splits, cand)
+    if k or w == 1:
+        return out
+    d = (out[2].to(torch.int64) * w).clamp(max=2**31 - 1).to(torch.int32)
+    return out[:2] + (torch.where(out[2] >= 0, d, out[2]),)
+
+
+def edit_wlev_argbest_staged(Q, T, weights, score_cutoff=0.0, exclude_self=False, self_shift=0, want_matrix=False, n_splits=None,
+                             to_index_base=0):
+    """Kernels only: per from-string the best to-string under rapidfuzz's Levenshtein.normalized_similarity(from, to,
+    weights=weights) (score 1 - D/M, key and cutoff as norm_lev).  Returns device (best_idx int32[n_from] (-1 = none;
+    + to_index_base otherwise), best_score float64[n_from], best_dist int32[n_from] = the weighted distance D, saturated at
+    2^31 - 1).  There is no distance matrix: want_matrix=True raises ValueError."""
+    if want_matrix:
+        raise ValueError("want_matrix=True: weighted Levenshtein has no distance matrix")
+    bi, bs, bd = _wlev_rows(Q, T, weights, score_cutoff, exclude_self, self_shift, 0, n_splits)
+    return _rebase(bi, to_index_base), bs, bd
+
+
+def edit_wlev_argbest(from_list, to_list, weights, score_cutoff=0.0, exclude_self=False, self_shift=0, want_matrix=False,
+                      n_splits=None, kept=None, reuse=False):
+    """Host lists in, device tensors out (see edit_wlev_argbest_staged); kept and reuse as in edit_argbest."""
+    check_weights(weights)
+    Q, T = _stage(from_list, to_list, kept, reuse)
+    return edit_wlev_argbest_staged(Q, T, weights, score_cutoff, exclude_self, self_shift, want_matrix, n_splits)
+
+
+def edit_wlev_topk_staged(Q, T, k, weights, score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, to_index_base=0):
+    """Kernels only: the k best to-strings per from-string under weighted Levenshtein, with the candidates and key of
+    edit_wlev_argbest_staged.  Returns device (idx int32[n_from, k] (-1 = empty slot; + to_index_base otherwise),
+    score float64[n_from, k] (0.0 in empty slots))."""
+    k = check_top_n(k)
+    idx, score = _wlev_rows(Q, T, weights, score_cutoff, exclude_self, self_shift, k, n_splits)
+    return _rebase(idx, to_index_base), score
+
+
+def edit_wlev_topk(from_list, to_list, k, weights, score_cutoff=0.0, exclude_self=False, self_shift=0, n_splits=None, kept=None,
+                   reuse=False):
+    """Host lists in, device tensors out (see edit_wlev_topk_staged); kept and reuse as in edit_argbest."""
+    k = check_top_n(k)
+    check_weights(weights)
+    Q, T = _stage(from_list, to_list, kept, reuse)
+    return edit_wlev_topk_staged(Q, T, k, weights, score_cutoff, exclude_self, self_shift, n_splits)
+
+
+def edit_wlev_cand_topk_staged(Q, T, cand, k, weights, score_cutoff=0.0, exclude_self=False, self_shift=0):
+    """Kernels only (pfz_wlev_rows in candidate mode): per from-row the k best to-strings among its candidates cand[i]
+    (check_candidates) under weighted Levenshtein.  k = 1 returns what edit_wlev_argbest_staged returns, k > 1 what
+    edit_wlev_topk_staged returns."""
+    k = check_top_n(k)
+    cand = check_candidates(cand, Q.n, T.n)
+    return _wlev_rows(Q, T, weights, score_cutoff, exclude_self, self_shift, 0 if k == 1 else k, cand=cand)
+
+
+def edit_wlev_cand_topk(from_list, to_list, cand, k, weights, score_cutoff=0.0, exclude_self=False, kept=None, reuse=False):
+    """Host lists in, device tensors out (see edit_wlev_cand_topk_staged); kept and reuse as in edit_argbest."""
+    k = check_top_n(k)
+    check_weights(weights)
+    Q, T = _stage(from_list, to_list, kept, reuse)
+    return edit_wlev_cand_topk_staged(Q, T, cand, k, weights, score_cutoff, exclude_self)

@@ -19,6 +19,12 @@ published known answers):
   * "dl" / "unrestricted_damerau_levenshtein" / "damerau_levenshtein_normalized_similarity" (unrestricted Damerau-Levenshtein,
     rapidfuzz.distance.DamerauLevenshtein's metric: a swapped pair may be edited again, so "CA" -> "ABC" costs 2;
     1 - dl / max(|a|, |b|), 0..1 scores like "levenshtein")             -> csrc/pfz_lev.cu (K3, dl_kernel, gated by OSA)
+  * functools.partial(<a callable that resolves to "levenshtein">, weights=(insertion, deletion, substitution)) -- rapidfuzz's
+    Levenshtein.normalized_similarity(from, to, weights=...): weighted Levenshtein, 1 - D / M on 0..1 like "levenshtein",
+    each weight an int in [0, 65535] (anything else is a ValueError); (w, w, w) scores as "levenshtein" -> csrc/pfz_lev.cu (K3,
+    wlev_kernel; DESIGN.md 4.17).  The partial may carry no positional arguments and no keyword but `weights`; every other
+    partial raises NotImplementedError.  A partial of DamerauLevenshtein.normalized_similarity resolves as Levenshtein (the rule
+    below), so it scores weighted Levenshtein where rapidfuzz itself would reject `weights`.
 The bare name "damerau_levenshtein" raises NotImplementedError: some libraries mean OSA by it, others unrestricted DL, so the
 user picks "osa" or "dl".
 A scorer may be given by name or as the rapidfuzz / jellyfish callable of that __name__.  A callable named
@@ -41,6 +47,7 @@ never scored, so the best edit-distance match can be missed: that is the trade (
 Deviations from the reference, both documented reference bugs (SURVEY.md 8a): a self-match excludes
 index i only (the reference mutates the shared to_list, _rapidfuzz.py:103-104), and the matcher can be
 reused for a two-list call after a self-match (`equal_lists` is per call)."""
+import functools
 from typing import Callable, List, Union
 
 import numpy as np
@@ -67,9 +74,13 @@ def _is_osa_module(module) -> bool:
 
 
 def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
-    """-> "ratio" | "norm_lev" | "norm_osa" | "norm_dl" | "jaro" | "jaro_winkler" (K3) or one of fuzzy.SCORER (K3b)."""
+    """-> "ratio" | "norm_lev" | "norm_osa" | "norm_dl" | "jaro" | "jaro_winkler" | "wlev" (K3) or one of fuzzy.SCORER (K3b).
+    A functools.partial is "wlev" (weighted Levenshtein, its weights from _scorer_weights) or, with weights None or (w, w, w),
+    "norm_lev"."""
     if scorer is None:
         scorer = default
+    if isinstance(scorer, functools.partial):
+        return "wlev" if editdist.uniform_weight(_scorer_weights(scorer, allow_jaro)) == 0 else "norm_lev"
     key = scorer.lower() if isinstance(scorer, str) else getattr(scorer, "__name__", "").lower()
     if key == "normalized_similarity" and not isinstance(scorer, str) and _is_osa_module(getattr(scorer, "__module__", None)):
         return "norm_osa"
@@ -87,17 +98,36 @@ def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
                               + "); polyfuzz_b200 has no CPU fallback")
 
 
-def _argbest(from_list, targets, metric, cutoff, self_match, distributed, kept=None, reuse=False):
+def _scorer_weights(scorer, allow_jaro=False):
+    """The validated `weights` (editdist.check_weights) of a partial scorer, None for any other scorer.  A partial is accepted
+    only when its func resolves to "norm_lev" by _resolve_scorer's rules and it has no positional arguments and no keyword
+    but `weights`; otherwise NotImplementedError."""
+    if not isinstance(scorer, functools.partial):
+        return None
+    try:
+        base = _resolve_scorer(scorer.func, None, allow_jaro)
+    except NotImplementedError:
+        base = None
+    if base != "norm_lev" or scorer.args or not set(scorer.keywords) <= {"weights"}:
+        raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation: a functools.partial is supported only as a "
+                                  "partial of Levenshtein.normalized_similarity with the keyword `weights` and no other "
+                                  "argument; polyfuzz_b200 has no CPU fallback")
+    return editdist.check_weights(scorer.keywords.get("weights"))
+
+
+def _argbest(from_list, targets, metric, cutoff, self_match, distributed, kept=None, reuse=False, weights=None):
     """Best to-string per from-string on this GPU, or -- distributed=True under torchrun -- on the to_list row-block of every
     rank followed by ONE all-gather of the per-shard bests and the canonical merge (score desc, global index asc): all ranks
     get the single-GPU result (SURVEY.md 8e; the reference's own fan-out is per from-row, polyfuzz/models/_rapidfuzz.py:92-95).
     kept / reuse: the matcher's kept to-side (editdist.KeptTargets; each rank keeps its own shard) and whether it may serve
-    this call."""
+    this call.  metric "wlev" scores weighted Levenshtein with `weights`."""
     comm = get_comm() if distributed else None
     token_scorer = metric in fuzzy.SCORER and metric != "ratio"
     if comm is None:
         if token_scorer:
             return fuzzy.fuzz_argbest(from_list, targets, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse) + (None,)
+        if metric == "wlev":
+            return editdist.edit_wlev_argbest(from_list, targets, weights, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
         return editdist.edit_argbest(from_list, targets, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
     lo, hi = shard_bounds(len(targets), comm.world_size, comm.rank)
     if token_scorer:
@@ -107,7 +137,11 @@ def _argbest(from_list, targets, metric, cutoff, self_match, distributed, kept=N
     else:
         Q = editdist.EditQueries(from_list)
         T = _shard_targets(targets[lo:hi], lo, kept, reuse)
-        bi, bs, bd = editdist.edit_argbest_staged(Q, T, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
+        if metric == "wlev":
+            bi, bs, bd = editdist.edit_wlev_argbest_staged(Q, T, weights, cutoff, exclude_self=self_match, self_shift=-lo,
+                                                           to_index_base=lo)
+        else:
+            bi, bs, bd = editdist.edit_argbest_staged(Q, T, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
     gi, gs, gd = comm.all_gather_best(bi, bs, bd)
     return editdist.lev_merge(gi, gs, gd)
 
@@ -119,7 +153,7 @@ def _shard_targets(shard, lo, kept, reuse):
     return kept.stage(("k3", lo), shard, lambda lst: editdist.EditTargets(lst), reuse)
 
 
-def _topk(from_list, targets, metric, cutoff, self_match, distributed, k, kept=None, reuse=False):
+def _topk(from_list, targets, metric, cutoff, self_match, distributed, k, kept=None, reuse=False, weights=None):
     """Top-k sibling of _argbest: the k best to-strings per from-string (device idx int32[n, k], -1 = empty slot, and score
     float64[n, k]) on this GPU, or -- distributed=True under torchrun -- per to_list row-block followed by ONE all-gather of the
     per-shard lists and the canonical merge, as TF-IDF and Embeddings do: all ranks get the single-GPU result."""
@@ -128,6 +162,8 @@ def _topk(from_list, targets, metric, cutoff, self_match, distributed, k, kept=N
     if comm is None:
         if token_scorer:
             return fuzzy.fuzz_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
+        if metric == "wlev":
+            return editdist.edit_wlev_topk(from_list, targets, k, weights, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
         return editdist.edit_topk(from_list, targets, k, metric, cutoff, exclude_self=self_match, kept=kept, reuse=reuse)
     lo, hi = shard_bounds(len(targets), comm.world_size, comm.rank)
     if token_scorer:
@@ -136,7 +172,11 @@ def _topk(from_list, targets, metric, cutoff, self_match, distributed, k, kept=N
     else:
         Q = editdist.EditQueries(from_list)
         T = _shard_targets(targets[lo:hi], lo, kept, reuse)
-        idx, val = editdist.edit_topk_staged(Q, T, k, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
+        if metric == "wlev":
+            idx, val = editdist.edit_wlev_topk_staged(Q, T, k, weights, cutoff, exclude_self=self_match, self_shift=-lo,
+                                                      to_index_base=lo)
+        else:
+            idx, val = editdist.edit_topk_staged(Q, T, k, metric, cutoff, exclude_self=self_match, self_shift=-lo, to_index_base=lo)
     gi, gv = comm.all_gather_topk(idx.contiguous(), val.contiguous())
     return merge_topk_any(gi, gv, k)
 
@@ -168,7 +208,7 @@ def _check_candidates(candidates, top_n, distributed):
     return candidates
 
 
-def _cand_topk(from_list, targets, metric, cutoff, self_match, k, candidates, to_list, re_train, kept):
+def _cand_topk(from_list, targets, metric, cutoff, self_match, k, candidates, to_list, re_train, kept, weights=None):
     """Candidate mode: TF-IDF's device top-n of every from-string, then the k best of those under the matcher's scorer.
     Returns host (idx int32[n, k], -1 = empty slot, score float64[n, k])."""
     cand, _, _ = candidates.match_arrays(from_list, to_list, re_train)
@@ -176,6 +216,9 @@ def _cand_topk(from_list, targets, metric, cutoff, self_match, k, candidates, to
     if token_scorer:
         idx, score = fuzzy.fuzz_cand_topk(from_list, targets, cand, k, metric, cutoff, exclude_self=self_match, kept=kept,
                                           reuse=not re_train)
+    elif metric == "wlev":
+        idx, score = editdist.edit_wlev_cand_topk(from_list, targets, cand, k, weights, cutoff, exclude_self=self_match, kept=kept,
+                                                  reuse=not re_train)[:2]
     else:
         idx, score = editdist.edit_cand_topk(from_list, targets, cand, k, metric, cutoff, exclude_self=self_match, kept=kept,
                                              reuse=not re_train)[:2]
@@ -199,6 +242,10 @@ class _KeepsTargets:
         if kept is None:
             kept = self._kept_targets = editdist.KeptTargets()
         return kept
+
+    def _weights_kw(self):
+        """The weighted-Levenshtein weights for _argbest / _topk / _cand_topk, passed only when the metric is "wlev"."""
+        return {"weights": self._weights} if self._metric == "wlev" else {}
 
     def __getstate__(self):
         st = dict(self.__dict__)
@@ -224,6 +271,7 @@ class RapidFuzz(_KeepsTargets, BaseMatcher):
         self.score_cutoff = score_cutoff * 100
         self.scorer = scorer
         self._metric = _resolve_scorer(scorer, "WRatio")
+        self._weights = _scorer_weights(scorer)
         self.equal_lists = False
         self.n_jobs = n_jobs
 
@@ -234,18 +282,20 @@ class RapidFuzz(_KeepsTargets, BaseMatcher):
         same as a fresh call's); any call that stages keeps its to-side."""
         self_match = to_list is None
         targets = from_list if self_match else to_list
-        unit = self._metric in ("norm_lev", "norm_osa", "norm_dl")             # scores already on 0..1
+        unit = self._metric in ("norm_lev", "norm_osa", "norm_dl", "wlev")     # scores already on 0..1
         scale = 1.0 if unit else 100.0
         cutoff = self.score_cutoff / 100.0 if unit else self.score_cutoff
         top_n = clip_top_n(self.top_n, to_list)
         if getattr(self, "candidates", None) is not None:
             idx, score = _cand_topk(from_list, targets, self._metric, cutoff, self_match, top_n, self.candidates, to_list, re_train,
-                                    self._kept())
+                                    self._kept(), **self._weights_kw())
             return _topk_frame(from_list, targets, idx, score / scale)
         if top_n > 1:
-            idx, score = _topk(from_list, targets, self._metric, cutoff, self_match, self.distributed, top_n, self._kept(), not re_train)
+            idx, score = _topk(from_list, targets, self._metric, cutoff, self_match, self.distributed, top_n, self._kept(), not re_train,
+                               **self._weights_kw())
             return _topk_frame(from_list, targets, idx.cpu().numpy(), score.cpu().numpy() / scale)
-        idx, score, _ = _argbest(from_list, targets, self._metric, cutoff, self_match, self.distributed, self._kept(), not re_train)
+        idx, score, _ = _argbest(from_list, targets, self._metric, cutoff, self_match, self.distributed, self._kept(), not re_train,
+                                 **self._weights_kw())
         idx = idx.cpu().numpy(); score = score.cpu().numpy() / scale
         to_arr = np.empty(len(targets) + 1, dtype=object); to_arr[:-1] = targets; to_arr[-1] = None
         sel = np.where(idx >= 0, idx, len(targets))
@@ -265,13 +315,17 @@ def _normalize_filled(idx, score):
 
 class EditDistance(_KeepsTargets, BaseMatcher):
     """Edit-distance matcher with the reference's EditDistance surface (n_jobs, scorer, model_id, normalize):
-    Similarity is the scorer's raw value (fuzz.ratio: 0..100, Levenshtein / OSA / DL / Jaro / Jaro-Winkler: 0..1) of the best to-string,
+    Similarity is the scorer's raw value (fuzz.ratio: 0..100, Levenshtein / weighted Levenshtein / OSA / DL / Jaro / Jaro-Winkler:
+    0..1) of the best to-string,
     min-max normalised over the column when `normalize` (polyfuzz/models/_distance.py:83-86).
     top_n (1..32): matches per from-string, clipped to the number of distinct to-strings when a to_list is given; an empty
     slot is (None, 0.0).  With top_n > 1, `normalize` takes ONE min and ONE max over every filled Similarity cell of the
     frame (empty slots excluded), so the first Similarity column can differ from the top_n = 1 frame's, whose min and max
     cover the best matches only; without `normalize` the first three columns are the top_n = 1 frame.
-    candidates (a TFIDF, top_n >= this top_n): score only its candidates per from-string (see the module docstring)."""
+    candidates (a TFIDF, top_n >= this top_n): score only its candidates per from-string (see the module docstring).
+    scorer may be functools.partial(Levenshtein.normalized_similarity, weights=(insertion, deletion, substitution)), rapidfuzz's
+    weighted Levenshtein (the one way to pass a rapidfuzz keyword through the reference's scorer(a, b) interface); see the module
+    docstring for the rules."""
 
     def __init__(self, n_jobs: int = 1, scorer: Union[str, Callable] = "ratio", model_id: str = None, normalize: bool = True,
                  distributed: bool = False, top_n: int = 1, candidates=None):
@@ -282,6 +336,7 @@ class EditDistance(_KeepsTargets, BaseMatcher):
         self.distributed = distributed
         self.scorer = scorer
         self._metric = _resolve_scorer(scorer, "ratio", allow_jaro=True)
+        self._weights = _scorer_weights(scorer, allow_jaro=True)
         self.normalize = normalize
         self.equal_lists = False
         self.n_jobs = n_jobs
@@ -300,13 +355,14 @@ class EditDistance(_KeepsTargets, BaseMatcher):
         if top_n > 1 or cand:
             if cand:
                 idx, score = _cand_topk(from_list, targets, self._metric, no_cut, self_match, top_n, self.candidates, to_list,
-                                        re_train, self._kept())
+                                        re_train, self._kept(), **self._weights_kw())
             else:
                 idx, score = _topk(from_list, targets, self._metric, no_cut, self_match, self.distributed, top_n, self._kept(),
-                                   not re_train)
+                                   not re_train, **self._weights_kw())
                 idx = idx.cpu().numpy(); score = score.cpu().numpy()
             return _topk_frame(from_list, targets, idx, _normalize_filled(idx, score) if self.normalize else score)
-        idx, score, _ = _argbest(from_list, targets, self._metric, no_cut, self_match, self.distributed, self._kept(), not re_train)
+        idx, score, _ = _argbest(from_list, targets, self._metric, no_cut, self_match, self.distributed, self._kept(), not re_train,
+                                 **self._weights_kw())
         idx = idx.cpu().numpy(); score = score.cpu().numpy()
         to_arr = np.empty(len(targets), dtype=object); to_arr[:] = targets
         matches = pd.DataFrame({"From": pd.Series(list(from_list), dtype=object), "To": pd.Series(to_arr[idx], dtype=object),
