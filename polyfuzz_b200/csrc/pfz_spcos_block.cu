@@ -256,7 +256,8 @@ __device__ __forceinline__ unsigned warp_sort_desc_u32(unsigned x, int lane) {
 //     the scan of tile t overlaps the table phase of tile t+1 (barrier A of t+1 is the one that protects the accumulators);
 //   * idle lanes of a partial chunk add into 32 dump words behind their row's cells (ptxas does not predicate ATOMS: a
 //     predicated red costs a divergent branch; a dump cell costs one select per item);
-//   * the item loop keeps B3_DEPTH posting chunks in flight per warp;
+//   * the item loop keeps B3_DEPTH posting chunks in flight per warp and loads each item's descriptor and first two table entries
+//     one item ahead, so no shared-memory load latency sits on the path from one item's updates to the next item's;
 //   * 16-bit mode: update = ceil(v16 * w15 / 2^16) placed in its half-word by one byte permute (IMAD + PRMT), v16 =
 //     max(1, floor(v * 2^16)), w15 = max(1, round(w * 2^15)) pre-packed with the word offset and the permute selector
 //     (pfz_index_pack_q15): -1.01 < update - v*w*2^15 < 2.01 units per product, >= 1 for every common term; margin 4 m + 2.
@@ -454,54 +455,67 @@ __device__ __forceinline__ uint2 lds64(unsigned a) {
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a));
     return v;
 }
+// e0, e1: the first two entries of the (row, weight) list, loaded by the caller ahead of time (entries past the list's end are
+// read but not used).
 template <bool P16>
-__device__ __forceinline__ void blk3_process(int lane, int cnt, unsigned fva, int nf, uint2 pk, unsigned acc_s, unsigned dump_s) {
+__device__ __forceinline__ void blk3_process(int lane, int cnt, unsigned fva, int nf, uint2 pk, uint2 e0, uint2 e1, unsigned acc_s,
+                                             unsigned dump_s) {
     unsigned cell, sel = 0u;
     const unsigned wq = pk.y;
     if (P16) { cell = acc_s + (pk.x & 0xffffu); sel = pk.x >> 16; }
     else cell = acc_s + (pk.x << 2);
     if (lane >= cnt) cell = dump_s;
-#pragma unroll 1
-    for (; nf >= 2; nf -= 2, fva += 16u) {
-        const uint2 e0 = lds64(fva), e1 = lds64(fva + 8u);
+    if (nf >= 2) {
         red_add_u32(cell + e0.x, blk3_update<P16>(e0.y, wq, sel));
         red_add_u32(cell + e1.x, blk3_update<P16>(e1.y, wq, sel));
-    }
-    if (nf) {
-        const uint2 e0 = lds64(fva);
+#pragma unroll 1
+        for (nf -= 2, fva += 16u; nf >= 2; nf -= 2, fva += 16u) {
+            const uint2 f0 = lds64(fva), f1 = lds64(fva + 8u);
+            red_add_u32(cell + f0.x, blk3_update<P16>(f0.y, wq, sel));
+            red_add_u32(cell + f1.x, blk3_update<P16>(f1.y, wq, sel));
+        }
+        if (nf) {
+            const uint2 f0 = lds64(fva);
+            red_add_u32(cell + f0.x, blk3_update<P16>(f0.y, wq, sel));
+        }
+    } else if (nf) {
         red_add_u32(cell + e0.x, blk3_update<P16>(e0.y, wq, sel));
     }
 }
 
-// The item phase of one unit as its own function (own register allocation): warp w walks items w, w + W, ... with the posting
-// chunks of the next B3_DEPTH items in flight.  items_s: shared address of the item array.  A slot behind the last item holds an
-// empty item (cnt = nf = 0).
+// The item phase of one unit as its own function (own register allocation): warp w walks items w, w + W, ... as a software
+// pipeline, so that no load's latency sits between an item's updates and the next item's:
+//   * the posting chunks of the next B3_DEPTH items are in flight (slot d: item i0 + d W);
+//   * the descriptor of the item that refills the slot next is loaded one item ahead, so the refill's posting load does not
+//     wait on a shared-memory load;
+//   * the first two (row, weight) entries of the next item are loaded before the current item's updates are issued.
+// items_s: shared address of the item array.  Past the last item a slot holds an empty item (cnt = nf = 0).
 template <int W, bool P16>
 __device__ __noinline__ void blk3_item_loop(unsigned items_s, int total, const uint2 *__restrict__ pk_lane, unsigned acc_s, unsigned dump_s) {
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    // {off, cnt, fva, nf}; an empty item's fva is the item array itself, so that its unused table entries are read from the arena
+    auto desc = [&](int i) { return i < total ? lds128(items_s + ((unsigned)i << 4)) : make_uint4(0u, 0u, items_s, 0u); };
+    auto post = [&](const uint4 &it) { return lane < (int)it.y ? __ldg(pk_lane + (int)it.x) : make_uint2(0u, 0u); };
     int qc[B3_DEPTH], qn[B3_DEPTH]; unsigned qa[B3_DEPTH]; uint2 qp[B3_DEPTH];
 #pragma unroll
     for (int d = 0; d < B3_DEPTH; ++d) {
-        const int i = w + d * W;
-        qc[d] = 0; qn[d] = 0; qa[d] = 0u; qp[d] = make_uint2(0u, 0u);
-        if (i < total) {
-            const uint4 it = lds128(items_s + ((unsigned)i << 4));            // {off, cnt, fva, nf}
-            qc[d] = (int)it.y; qn[d] = (int)it.w; qa[d] = it.z;
-            if (lane < (int)it.y) qp[d] = __ldg(pk_lane + (int)it.x);
-        }
+        const uint4 it = desc(w + d * W);
+        qc[d] = (int)it.y; qn[d] = (int)it.w; qa[d] = it.z; qp[d] = post(it);
     }
+    uint4 nx = desc(w + B3_DEPTH * W);                                   // the item that refills slot 0
+    uint2 e0 = lds64(qa[0]), e1 = lds64(qa[0] + 8u);                   // first entries of slot 0's item
 #pragma unroll 1
     for (int i0 = w; i0 < total; i0 += B3_DEPTH * W) {
 #pragma unroll
         for (int d = 0; d < B3_DEPTH; ++d) {
-            blk3_process<P16>(lane, qc[d], qa[d], qn[d], qp[d], acc_s, dump_s);
-            const int ni = i0 + (d + B3_DEPTH) * W;
-            qc[d] = 0; qn[d] = 0; qp[d] = make_uint2(0u, 0u);
-            if (ni < total) {
-                const uint4 it = lds128(items_s + ((unsigned)ni << 4));
-                qc[d] = (int)it.y; qn[d] = (int)it.w; qa[d] = it.z;
-                if (lane < (int)it.y) qp[d] = __ldg(pk_lane + (int)it.x);
-            }
+            const int n = (d + 1) % B3_DEPTH;                            // the slot of the next item
+            const int cc = qc[d], cn = qn[d]; const unsigned ca = qa[d]; const uint2 cp = qp[d];
+            qc[d] = (int)nx.y; qn[d] = (int)nx.w; qa[d] = nx.z; qp[d] = post(nx);
+            nx = desc(i0 + (d + B3_DEPTH + 1) * W);
+            const unsigned na = qa[n];
+            const uint2 f0 = lds64(na), f1 = lds64(na + 8u);
+            blk3_process<P16>(lane, cc, ca, cn, cp, e0, e1, acc_s, dump_s);
+            e0 = f0; e1 = f1;
         }
     }
 }
@@ -733,7 +747,8 @@ __global__ void __launch_bounds__(BF * 32, PFZ_B3_MIN_CTAS(BF)) spcos_blk3_kerne
                     for (int c = 0; c < len; c += 32) {
                         uint2 pk = make_uint2(0u, 0u);
                         if (lane < len - c) pk = __ldg(pk_lane + s + c);
-                        blk3_process<P16>(lane, len - c, fv_s + ((fvd >> 5) << 3), (int)(fvd & 31u), pk, acc_s, dump_s);
+                        const unsigned fva = fv_s + ((fvd >> 5) << 3);
+                        blk3_process<P16>(lane, len - c, fva, (int)(fvd & 31u), pk, lds64(fva), lds64(fva + 8u), acc_s, dump_s);
                     }
                 }
             }
