@@ -41,6 +41,13 @@ extern "C" {
 #define PFZ_METRIC_NORM_OSA  7     /* 1 - osa/max(|a|,|b|)                                         */
 #define PFZ_METRIC_DL        8     /* unrestricted Damerau-Levenshtein distance                    */
 #define PFZ_METRIC_NORM_DL   9     /* 1 - dl/max(|a|,|b|)                                          */
+/* 10 is unassigned: the id weighted Levenshtein left free when it took its own entry point (pfz_wlev_rows); pfz_lev_rows
+ * rejects it as an unknown metric.  11..15: rapidfuzz 3.x normalised similarities 1 - d/M (1 when M = 0), a = from-string. */
+#define PFZ_METRIC_NORM_INDEL   11 /* Indel: d = |a|+|b|-2*LCS, M = |a|+|b| (RATIO's ns, without the x100)  */
+#define PFZ_METRIC_NORM_LCSSEQ  12 /* LCSseq: d = M - LCS, M = max(|a|,|b|)                                */
+#define PFZ_METRIC_NORM_HAMMING 13 /* Hamming, pad=True: d = mismatches below min(|a|,|b|) + ||a|-|b||, M = max */
+#define PFZ_METRIC_NORM_PREFIX  14 /* Prefix: d = M - common prefix length, M = max(|a|,|b|)                */
+#define PFZ_METRIC_NORM_POSTFIX 15 /* Postfix: d = M - common suffix length, M = max(|a|,|b|)               */
 
 int         pfz_abi_version(void);
 const char *pfz_last_error(void);
@@ -245,18 +252,21 @@ int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32
  * 1/2/4/8/16 -> length <= 64*n_words) against the to-strings, with a fused per-row epilogue.
  * Replaces: rapidfuzz process.extractOne / process.extract(query, to_list, scorer, limit=k) and the scorer loop of
  *           polyfuzz/models/_distance.py:98-99 (np.argmax, or the sort of the scorer values for top-k).
- *   metric: PFZ_METRIC_*; for NORM_LEV / JARO / JARO_WINKLER / NORM_OSA / NORM_DL a candidate needs score >= score_cutoff; for RATIO
+ *   metric: PFZ_METRIC_*; for NORM_LEV / JARO / JARO_WINKLER / NORM_OSA / NORM_DL / NORM_INDEL .. NORM_POSTFIX a candidate needs
+ *           score >= score_cutoff (one step); for RATIO
  *           rapidfuzz's two steps: ns = 1 - indel/(|a|+|b|) >= score_cutoff/100 (fuzz.ratio) and score = ns*100 >= score_cutoff
  *           (extractOne), which differ whenever (ns*100)/100 != ns -- e.g. ns = 17/25 is rejected at score_cutoff 68.0; the raw
  *           distances LEV, INDEL, OSA and DL have no cutoff (best = smallest)
  *   exclude_self: skip to-row == from-row + self_shift
  *   key: score desc, to-index asc (ties -> lowest to-index)
  *   k (epilogue): 0 = arg-best: part_idx / part_score / part_dist [n_splits][n_from] partial bests (merge with pfz_lev_merge);
- *           part_dist holds the distance, or for JARO / JARO_WINKLER the number of matching characters; empty (-1, 0.0, -1).
+ *           part_dist holds the distance (NORM_INDEL .. NORM_POSTFIX: their d), or for JARO / JARO_WINKLER the number of matching
+ *           characters; empty (-1, 0.0, -1).
  *           1..32 = top-k: part_idx / part_score [n_splits][n_from][k] sorted lists, empty slots (-1, 0.0) (merge with
- *           pfz_topk_merge); metric NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA or NORM_DL; part_dist and matrix NULL.
+ *           pfz_topk_merge); metric NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA, NORM_DL or NORM_INDEL .. NORM_POSTFIX; part_dist
+ *           and matrix NULL.
  *   matrix (arg-best, may be NULL): int32 [n_from][matrix_ld] full distance matrix (Levenshtein, Indel, OSA for OSA / NORM_OSA, DL
- *           for DL / NORM_DL); must be NULL for JARO / JARO_WINKLER, and needs gate == NULL
+ *           for DL / NORM_DL); must be NULL for JARO / JARO_WINKLER and NORM_INDEL .. NORM_POSTFIX, and needs gate == NULL
  *   gate (DL / NORM_DL only, may be NULL): float64[n_from], per from-row a proven lower bound of its k-th best score (k = 1 for the
  *           arg-best) over the row's to-strings; pairs whose score upper bound is below it are skipped.  The k-th best OSA score of
  *           the row (this call with OSA / NORM_OSA and the same cutoff, exclusion and k, merged over the splits) is such a bound,
@@ -274,6 +284,8 @@ int pfz_lev_pack(const uint32_t *to_blob, const int64_t *to_offsets, const int32
  * pair may be edited again (dl("CA", "ABC") = 2); NORM_DL = 1 - dl/max(|a|,|b|); DESIGN.md 4.10 gives the bounds and the kernel.
  * JARO / JARO_WINKLER: jellyfish's definition on code points, from-string first (the reference calls
  * scorer(from_string, to_string), polyfuzz/models/_distance.py:98); DESIGN.md 4.5 gives the recurrence.
+ * NORM_INDEL / NORM_LCSSEQ run the bit-parallel LCS recurrence of RATIO; NORM_HAMMING / NORM_PREFIX / NORM_POSTFIX compare symbol
+ * by symbol, 4 per step (DESIGN.md 4.18).
  * n_ids <= 0 (or n_to < 0) returns 0 without launching anything.                                                          */
 int pfz_lev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t n_from, const int32_t *from_ids, int32_t n_ids,
                  int32_t n_words, const uint8_t *sym_table, const uint32_t *packed, const int64_t *grp_word_off,

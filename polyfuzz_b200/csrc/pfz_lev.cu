@@ -1,5 +1,5 @@
-// pfz_lev.cu -- K3: all-pairs edit distance (bit-parallel Myers/Hyyro Levenshtein and Hyyro LCS/Indel) and
-// Jaro / Jaro-Winkler similarity over the |from| x |to| grid with a fused per-row arg-best.
+// pfz_lev.cu -- K3: all-pairs edit distance (bit-parallel Myers/Hyyro Levenshtein and Hyyro LCS/Indel/LCSseq), Jaro /
+// Jaro-Winkler and the positional Hamming / Prefix / Postfix similarities over the |from| x |to| grid with a fused per-row arg-best.
 //
 // Replaces rapidfuzz's scorer loop as the reference calls it:
 //     polyfuzz/models/_rapidfuzz.py:99-113  process.extractOne(q, to_list, score_cutoff, scorer=fuzz.ratio)
@@ -78,6 +78,10 @@ __device__ __forceinline__ double ratio_ns(int d, int la, int lb) {      // Inde
     const int m = la + lb;
     return m ? 1.0 - (double)d / (double)m : 1.0;
 }
+
+// Normalised similarity of the sequence metrics NORM_INDEL .. NORM_POSTFIX: rapidfuzz's 1 - d / M with the distance d and the
+// maximum M, in NORM_LEV's order of operations (float64, 1 when M = 0).
+__device__ __forceinline__ double seq_score(int d, int mx) { return mx ? 1.0 - (double)d / (double)mx : 1.0; }
 
 __device__ __forceinline__ double score_of(int metric, int d, int la, int lb) {
     if (metric == PFZ_METRIC_NORM_LEV) { const int m = max(la, lb); return m ? 1.0 - (double)d / (double)m : 1.0; }
@@ -233,10 +237,13 @@ __device__ __forceinline__ int lcs_length(const W *peq, const uint32_t *src, int
 // string alignment (LevColumn); LCS = true: longest common subsequence (Hyyro 2004) -> Indel = la + lb - 2*LCS.
 // TOPK = false: per-row arg-best; TOPK = true: the k best per row in a WarpTopK, offered after every group of 32 to-strings.
 // CAND = true: the row's candidate list instead of the split's to-groups (to_steps / to_pos / to_column of pfz_common.cuh).
+// SEQ = true (with LCS): the epilogue of NORM_INDEL / NORM_LCSSEQ (seq_score) instead of RATIO / INDEL's; a template parameter,
+// so the existing instantiations keep their code.
 // (minimum 1 block per SM for TOPK: without it ptxas's register target makes some top-k classes spill; 0 = unspecified)
-template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false, bool OSA = false, bool CAND = false>
+template <typename W, int NW, bool LCS, int WARPS, bool TOPK = false, bool OSA = false, bool CAND = false, bool SEQ = false>
 __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const LevParams P) {
     static_assert(!(OSA && LCS), "OSA extends the Levenshtein recurrence");
+    static_assert(!SEQ || LCS, "the Indel / LCSseq epilogue reads the LCS recurrence");
     constexpr int B = WordOps<W>::BITS;
     extern __shared__ __align__(16) unsigned char dyn[];
     const int lane = lane_id();
@@ -299,7 +306,16 @@ __global__ void __launch_bounds__(WARPS * 32, TOPK ? 1 : 0) lev_kernel(const Lev
                 }
                 dist = m + n - 2 * lcs;
             }
-            if (have) {
+            if constexpr (SEQ) {
+                if (have) {                             // NORM_INDEL: d = indel, M = m + n; NORM_LCSSEQ: d = M - LCS, M = max(m, n)
+                    const int mx = P.metric == PFZ_METRIC_NORM_INDEL ? m + n : max(m, n);
+                    const int d = P.metric == PFZ_METRIC_NORM_INDEL ? dist : mx - (m + n - dist) / 2;
+                    const double sc = seq_score(d, mx);
+                    const bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) && sc >= P.cutoff;
+                    if constexpr (TOPK) { cand_s = sc; cand_j = ok ? orig : -1; }
+                    else if (ok) best.offer(sc, orig, d);
+                }
+            } else if (have) {
                 if (P.matrix) P.matrix[(int64_t)i * P.matrix_ld + orig] = dist;
                 bool ok = !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift);
                 double sc;
@@ -438,6 +454,105 @@ __global__ void __launch_bounds__(WARPS * 32) jaro_kernel(const LevParams P) {
                 else if (ok) best.offer(sc, orig, k);
             }
             if constexpr (TOPK) top.offer(cand_s, cand_j);
+        }
+        store_row<TOPK>(P, i, top, best);
+        __syncwarp();
+    }
+}
+
+// ---- positional metrics: Hamming, Prefix, Postfix (DESIGN.md 4.18) ----------------------------------------------------------
+// No recurrence: the lane's to-string is compared with the pattern 4 symbols per step.  The pattern sits in shared memory as the
+// packed to-side stores a string (symbol q in byte q % 4 of word q / 4), behind one zero guard word and followed by another, so
+// Postfix can funnel-shift a pattern word into line with any text word.  Comparisons are masked by the two lengths, never by the
+// padding bytes.  A text symbol 0 (a code point outside the batch's alphabet) never equals a pattern symbol (1..255), so
+// alphabet batches need nothing more.
+constexpr int POS_WORDS = 1024 / 4 + 2;                 // the longest pattern of the word classes, and the two guards
+
+// the warp's pattern: pw[0] and pw[ceil(m / 4) + 1] zero, pw[1 + w] symbols 4w .. 4w + 3 (zero past m)
+__device__ __forceinline__ void stage_pattern(uint32_t *pw, const uint32_t *cps, int m, const uint8_t *sym_table) {
+    const int nw = (m + 3) >> 2;
+    for (int w = lane_id(); w < nw; w += 32) {
+        uint32_t word = 0;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+            const int q = 4 * w + b;
+            if (q < m) { const uint32_t c = cps[q]; word |= (uint32_t)(c < 0x110000u ? sym_table[c] : 0) << (8 * b); }
+        }
+        pw[w + 1] = word;
+    }
+    if (lane_id() == 0) { pw[0] = 0; pw[nw + 1] = 0; }
+    __syncwarp();
+}
+
+// mismatches at positions < L (= min(m, n)); text word w lies at src[32 w]
+__device__ __forceinline__ int hamming_mismatches(const uint32_t *pw, const uint32_t *src, int L) {
+    int bits = 0;
+#pragma unroll 4
+    for (int w = 0; 4 * w < L; ++w) {
+        uint32_t ne = __vcmpne4(src[(size_t)w * 32], pw[w + 1]);                 // 0xff per differing byte
+        if (4 * w + 4 > L) ne &= 0xffffffffu >> (8 * (4 * w + 4 - L));         // positions >= L
+        bits += __popc(ne);
+    }
+    return bits >> 3;
+}
+
+// length of the common prefix, at most L
+__device__ __forceinline__ int common_prefix(const uint32_t *pw, const uint32_t *src, int L) {
+    for (int w = 0; 4 * w < L; ++w) {
+        const uint32_t ne = __vcmpne4(src[(size_t)w * 32], pw[w + 1]);
+        if (ne) return min(4 * w + ((__ffs(ne) - 1) >> 3), L);
+    }
+    return L;
+}
+
+// length of the common suffix of the pattern (m symbols) and the text (n symbols), at most L = min(m, n): text words from the
+// last one down; text position j faces pattern position j + m - n
+__device__ __forceinline__ int common_suffix(const uint32_t *pw, const uint32_t *src, int m, int n, int L) {
+    for (int w = (n - 1) >> 2; 4 * w + 3 >= n - L; --w) {
+        const int q = 4 * w + m - n;                    // pattern position of the word's byte 0, >= -3
+        const int idx = (q + 4) >> 2;                   // pw index of the word holding position q (guard word 0 for q < 0)
+        const uint32_t pat = __funnelshift_r(pw[idx], pw[idx + 1], 8 * (q & 3));
+        uint32_t ne = __vcmpne4(src[(size_t)w * 32], pat);
+        if (4 * w + 4 > n) ne &= 0xffffffffu >> (8 * (4 * w + 4 - n));         // positions >= n
+        if (ne) return min(n - 1 - (4 * w + ((31 - __clz(ne)) >> 3)), L);
+    }
+    return L;
+}
+
+// NORM_HAMMING (pad: d = mismatches below min(m, n) + |m - n|), NORM_PREFIX and NORM_POSTFIX (d = M - the common length);
+// M = max(m, n).  The metric branch is warp-uniform.  (minimum 1 block per SM: without it ptxas aims at 32 registers and the
+// arg-best spills)
+template <int WARPS, bool TOPK, bool CAND>
+__global__ void __launch_bounds__(WARPS * 32, 1) pos_kernel(const LevParams P) {
+    extern __shared__ __align__(16) unsigned char dyn[];
+    uint32_t *pw = reinterpret_cast<uint32_t *>(dyn) + (size_t)(threadIdx.x >> 5) * POS_WORDS;
+    const GroupRange gr = to_steps<CAND>(P.n_to, P.n_splits, P.cand);
+
+    for (;;) {
+        const int i = claim_row(P.counter + blockIdx.y, P.from_ids, P.n_ids);
+        if (i < 0) break;
+        const int64_t fb = P.from_off[i];
+        const int m = (int)(P.from_off[i + 1] - fb);
+        stage_pattern(pw, P.from_blob + fb, m, P.sym_table);
+
+        WarpArgBest<> best;
+        WarpTopK top;
+        if constexpr (TOPK) top.init(P.k); else best.init();
+        for (int g = gr.lo; g < gr.hi; ++g) {
+            const int p = to_pos<CAND>(g, i, P.cand);
+            const bool have = to_have<CAND>(p, P.n_to);
+            const int n = have ? P.slen[p] : 0;
+            const int orig = have ? P.sorig[p] : -1;
+            const uint32_t *src = to_column<CAND>(P.packed, P.grp_word_off, g, p);
+            const int L = min(m, n), mx = max(m, n);
+            int d;
+            if (P.metric == PFZ_METRIC_NORM_HAMMING) d = hamming_mismatches(pw, src, L) + (mx - L);
+            else if (P.metric == PFZ_METRIC_NORM_PREFIX) d = mx - common_prefix(pw, src, L);
+            else d = mx - (L > 0 ? common_suffix(pw, src, m, n, L) : 0);
+            const double sc = seq_score(d, mx);
+            const bool ok = have && !(P.exclude_self && (int64_t)orig == (int64_t)i + P.self_shift) && sc >= P.cutoff;
+            if constexpr (TOPK) top.offer(sc, ok ? orig : -1);
+            else if (ok) best.offer(sc, orig, d);
         }
         store_row<TOPK>(P, i, top, best);
         __syncwarp();
@@ -831,10 +946,16 @@ static int dispatch_words(int n_words, F &&f) {
     }
 }
 
-// word class -> kernel instantiation; the metric picks Levenshtein, Indel, OSA, Jaro or DL (gate: DL only)
+// word class -> kernel instantiation; the metric picks Levenshtein, Indel, OSA, Jaro, DL (gate: DL only) or a sequence metric
 template <bool TOPK, bool CAND>
 static int launch_class(const LevParams &P, const double *gate, int n_words, int sms, cudaStream_t st) {
     const int mt = P.metric;
+    if (mt == PFZ_METRIC_NORM_HAMMING || mt == PFZ_METRIC_NORM_PREFIX || mt == PFZ_METRIC_NORM_POSTFIX) {
+        // one instantiation for every word class: the pattern takes POS_WORDS words (1 KB) per warp
+        constexpr int WARPS = 4;
+        return launch_rows(pos_kernel<WARPS, TOPK, CAND>, WARPS, (size_t)WARPS * POS_WORDS * sizeof(uint32_t), P.n_ids, P.n_splits,
+                           sms, st, P);
+    }
     return dispatch_words(n_words, [&](auto c) {
         using W = typename decltype(c)::Word;
         constexpr int NW = decltype(c)::N;
@@ -858,6 +979,8 @@ static int launch_class(const LevParams &P, const double *gate, int n_words, int
             return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK, true, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
         if (mt == PFZ_METRIC_INDEL || mt == PFZ_METRIC_RATIO)
             return launch_rows(lev_kernel<W, NW, true, WARPS, TOPK, false, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
+        if (mt == PFZ_METRIC_NORM_INDEL || mt == PFZ_METRIC_NORM_LCSSEQ)
+            return launch_rows(lev_kernel<W, NW, true, WARPS, TOPK, false, CAND, true>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
         return launch_rows(lev_kernel<W, NW, false, WARPS, TOPK, false, CAND>, WARPS, smem, P.n_ids, P.n_splits, sms, st, P);
     });
 }
@@ -905,7 +1028,8 @@ int pfz_lev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
                  int32_t n_splits, int32_t k, const int32_t *cand_idx, int32_t c, const int32_t *pos_of, int32_t *part_idx,
                  double *part_score, int32_t *part_dist, int32_t *matrix, int64_t matrix_ld, const double *gate, int32_t *counter,
                  void *stream) {
-    PFZ_REQUIRE(metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_DL, "pfz_lev_rows: unknown metric %d", metric);
+    const bool seq = metric >= PFZ_METRIC_NORM_INDEL && metric <= PFZ_METRIC_NORM_POSTFIX;
+    PFZ_REQUIRE((metric >= PFZ_METRIC_LEV && metric <= PFZ_METRIC_NORM_DL) || seq, "pfz_lev_rows: unknown metric %d", metric);
     PFZ_REQUIRE(n_words == 0 || n_words == 1 || n_words == 2 || n_words == 4 || n_words == 8 || n_words == 16,
                 "pfz_lev_rows: n_words %d unsupported (0 = 32-bit word, 1, 2, 4, 8, 16 64-bit words)", n_words);
     PFZ_REQUIRE(k >= 0 && k <= 32, "pfz_lev_rows: k=%d unsupported (0 = arg-best, 1..32 = top-k)", k);
@@ -913,13 +1037,15 @@ int pfz_lev_rows(const uint32_t *from_blob, const int64_t *from_offsets, int32_t
     const bool dl = metric == PFZ_METRIC_DL || metric == PFZ_METRIC_NORM_DL;
     if (k >= 1) {
         PFZ_REQUIRE((metric >= PFZ_METRIC_NORM_LEV && metric <= PFZ_METRIC_JARO_WINKLER) || metric == PFZ_METRIC_NORM_OSA ||
-                    metric == PFZ_METRIC_NORM_DL,
-                    "pfz_lev_rows: top-k metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA, NORM_DL)", metric);
+                    metric == PFZ_METRIC_NORM_DL || seq,
+                    "pfz_lev_rows: top-k metric %d unsupported (NORM_LEV, RATIO, JARO, JARO_WINKLER, NORM_OSA, NORM_DL, NORM_INDEL .. "
+                    "NORM_POSTFIX)", metric);
         PFZ_REQUIRE(!part_dist && !matrix, "pfz_lev_rows: top-k has no distance output (part_dist and matrix must be NULL)");
     } else {
         PFZ_REQUIRE(part_dist, "pfz_lev_rows: arg-best needs part_dist");
     }
     PFZ_REQUIRE(!(jaro && matrix), "pfz_lev_rows: the distance matrix is not available for the Jaro metrics (matrix must be NULL)");
+    PFZ_REQUIRE(!(seq && matrix), "pfz_lev_rows: the distance matrix is not available for metric %d (matrix must be NULL)", metric);
     PFZ_REQUIRE(!gate || dl, "pfz_lev_rows: gate is for DL / NORM_DL only (gate must be NULL for metric %d)", metric);
     PFZ_REQUIRE(!(matrix && gate), "pfz_lev_rows: the distance matrix needs every pair, so gate must be NULL with a matrix");
     if (cand_idx)

@@ -13,6 +13,14 @@ polyfuzz/models/_distance.py:89-102) and rapidfuzz's published definitions:
     "norm_dl"   DamerauLevenshtein.normalized_similarity = 1 - dl/max(|a|,|b|)  in [0, 1]
     "dl"        raw unrestricted Damerau-Levenshtein distance (Lowrance-Wagner, unit costs: a swapped pair may be edited
                 again, so dl("CA", "ABC") = 2); gated by an OSA pass (DESIGN.md 4.10)
+    The sequence metrics, rapidfuzz 3.x's normalized_similarity = 1 - d/M (1.0 when M = 0), in [0, 1]; best_dist is d:
+    "norm_indel"    Indel:   d = |a| + |b| - 2 LCS, M = |a| + |b|  (fuzz.ratio's ns, without its x100)
+    "norm_lcsseq"   LCSseq:  d = M - LCS, M = max(|a|, |b|)
+    "norm_hamming"  Hamming with pad=True (rapidfuzz 3's default; rapidfuzz 2 raises on unequal lengths): d = mismatches at the
+                    positions both strings have + ||a| - |b||, M = max(|a|, |b|)
+    "norm_prefix"   Prefix:  d = M - the common prefix length, M = max(|a|, |b|)
+    "norm_postfix"  Postfix: d = M - the common suffix length, M = max(|a|, |b|)
+    They take norm_lev's one-step cutoff (score >= score_cutoff) and have no distance matrix (DESIGN.md 4.18).
 The Jaro metrics are computed on code points, from-string first (the reference calls scorer(from_string, to_string),
 polyfuzz/models/_distance.py:98); their best_dist is the number of matching characters, and they have no distance
 matrix (want_matrix=True raises ValueError).
@@ -41,8 +49,9 @@ from .engine import _dev, _p, _stream, _to_dev, topk_merge
 from .strings import pack_strings
 
 METRIC = {"lev": 0, "indel": 1, "norm_lev": 2, "ratio": 3, "jaro": 4, "jaro_winkler": 5, "osa": 6, "norm_osa": 7, "dl": 8,
-          "norm_dl": 9}
+          "norm_dl": 9, "norm_indel": 11, "norm_lcsseq": 12, "norm_hamming": 13, "norm_prefix": 14, "norm_postfix": 15}
 JARO_METRICS = ("jaro", "jaro_winkler")
+SEQ_METRICS = ("norm_indel", "norm_lcsseq", "norm_hamming", "norm_prefix", "norm_postfix")
 # DL metric -> the OSA metric whose k-th best score gates it (norm_osa <= norm_dl pair by pair, DESIGN.md 4.10)
 DL_GATE = {"dl": "osa", "norm_dl": "norm_osa"}
 N_CODE_POINTS = 0x110000
@@ -289,7 +298,7 @@ def edit_argbest_staged(Q, T, metric="ratio", score_cutoff=0.0, exclude_self=Fal
     best_dist int32[n_from] [, matrix int32[n_from, n_to]]) as device tensors.
     dl / norm_dl: per word class an OSA arg-best pass and its split merge give each row's gate, then the DL pass;
     dl_gate=False (for timing) skips the OSA pass, and a matrix is computed without it."""
-    if want_matrix and metric in JARO_METRICS:
+    if want_matrix and (metric in JARO_METRICS or metric in SEQ_METRICS):
         raise ValueError(f"want_matrix=True: the {metric!r} metric has no integer distance matrix")
     matrix = torch.zeros((max(Q.n, 1), max(T.n, 1)), dtype=torch.int32, device=_dev()) if want_matrix else None
     bi, bs, bd = _edit_rows(Q, T, metric, score_cutoff, exclude_self, self_shift, 0, n_splits, matrix=matrix, dl_gate=dl_gate)
@@ -314,7 +323,7 @@ def edit_argbest(from_list, to_list, metric="ratio", score_cutoff=0.0, exclude_s
 
 
 TOPK_MAX = 32
-TOPK_METRICS = ("norm_lev", "ratio", "jaro", "jaro_winkler", "norm_osa", "norm_dl")
+TOPK_METRICS = ("norm_lev", "ratio", "jaro", "jaro_winkler", "norm_osa", "norm_dl") + SEQ_METRICS
 
 
 def check_top_n(k):

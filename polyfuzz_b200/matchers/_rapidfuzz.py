@@ -19,6 +19,13 @@ published known answers):
   * "dl" / "unrestricted_damerau_levenshtein" / "damerau_levenshtein_normalized_similarity" (unrestricted Damerau-Levenshtein,
     rapidfuzz.distance.DamerauLevenshtein's metric: a swapped pair may be edited again, so "CA" -> "ABC" costs 2;
     1 - dl / max(|a|, |b|), 0..1 scores like "levenshtein")             -> csrc/pfz_lev.cu (K3, dl_kernel, gated by OSA)
+  * rapidfuzz.distance's other normalised similarities, 1 - d / M on 0..1 like "levenshtein" (DESIGN.md 4.18):
+    "indel" / "indel_normalized_similarity" (d = |a| + |b| - 2 LCS, M = |a| + |b|: fuzz.ratio / 100 without the rounding of the
+    round trip), "lcsseq" / "lcs_seq" / "lcsseq_normalized_similarity" / "lcs_seq_normalized_similarity" (d = M - LCS),
+    "hamming" / "hamming_normalized_similarity" (rapidfuzz 3's pad=True: unequal lengths count the surplus as mismatches, where
+    rapidfuzz 2 raises), "prefix" / "prefix_normalized_similarity" and "postfix" / "postfix_normalized_similarity" (d = M - the
+    common prefix / suffix length); M = max(|a|, |b|) but for Indel
+                                                                         -> csrc/pfz_lev.cu (K3, lev_kernel's LCS / pos_kernel)
   * functools.partial(<a callable that resolves to "levenshtein">, weights=(insertion, deletion, substitution)) -- rapidfuzz's
     Levenshtein.normalized_similarity(from, to, weights=...): weighted Levenshtein, 1 - D / M on 0..1 like "levenshtein",
     each weight an int in [0, 65535] (anything else is a ValueError); (w, w, w) scores as "levenshtein" -> csrc/pfz_lev.cu (K3,
@@ -29,9 +36,10 @@ The bare name "damerau_levenshtein" raises NotImplementedError: some libraries m
 user picks "osa" or "dl".
 A scorer may be given by name or as the rapidfuzz / jellyfish callable of that __name__.  A callable named
 `normalized_similarity` is OSA when a dotted component of its __module__ is "osa" or starts with "osa_" (case-insensitive, e.g.
-rapidfuzz.distance.OSA), and normalised Levenshtein otherwise -- including rapidfuzz.distance.DamerauLevenshtein's, which
-therefore scores Levenshtein, not DL; pointing it at "dl" changes what an existing call returns, so it is left to a separate
-fix.  These rules are written from rapidfuzz's documented module layout;
+rapidfuzz.distance.OSA), and normalised Levenshtein otherwise -- including rapidfuzz.distance.DamerauLevenshtein's, Indel's,
+LCSseq's, Hamming's, Prefix's and Postfix's, which therefore score Levenshtein; pointing them at their own metrics changes what an
+existing call returns, so it is left to a separate fix, and the names above are the way to these scorers.  These rules are
+written from rapidfuzz's documented module layout;
 rapidfuzz is not a dependency, so its callables' actual __name__ / __module__ values are not checked by the tests, which use
 stand-in functions.  Arbitrary Python callables cannot be compiled to the device and raise NotImplementedError -- there is no
 CPU fallback.
@@ -61,7 +69,11 @@ from ..distributed import get_comm, merge_topk_any, shard_bounds
 _NAMES = {"ratio": "ratio", "levenshtein": "norm_lev", "norm_lev": "norm_lev", "normalized_similarity": "norm_lev",
           "normalized_levenshtein": "norm_lev", "osa": "norm_osa", "optimal_string_alignment": "norm_osa",
           "osa_normalized_similarity": "norm_osa", "dl": "norm_dl", "unrestricted_damerau_levenshtein": "norm_dl",
-          "damerau_levenshtein_normalized_similarity": "norm_dl"}
+          "damerau_levenshtein_normalized_similarity": "norm_dl", "indel": "norm_indel", "indel_normalized_similarity": "norm_indel",
+          "lcsseq": "norm_lcsseq", "lcs_seq": "norm_lcsseq", "lcsseq_normalized_similarity": "norm_lcsseq",
+          "lcs_seq_normalized_similarity": "norm_lcsseq", "hamming": "norm_hamming", "hamming_normalized_similarity": "norm_hamming",
+          "prefix": "norm_prefix", "prefix_normalized_similarity": "norm_prefix", "postfix": "norm_postfix",
+          "postfix_normalized_similarity": "norm_postfix"}
 _FUZZ = {k.lower(): k for k in fuzzy.SCORER if k != "ratio"}
 # jellyfish's function names (and short forms); 0..1 scores, so only EditDistance takes them
 _JARO = {"jaro": "jaro", "jaro_similarity": "jaro", "jaro_winkler": "jaro_winkler", "jaro_winkler_similarity": "jaro_winkler"}
@@ -74,7 +86,8 @@ def _is_osa_module(module) -> bool:
 
 
 def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
-    """-> "ratio" | "norm_lev" | "norm_osa" | "norm_dl" | "jaro" | "jaro_winkler" | "wlev" (K3) or one of fuzzy.SCORER (K3b).
+    """-> "ratio" | "norm_lev" | "norm_osa" | "norm_dl" | "jaro" | "jaro_winkler" | "wlev" | one of editdist.SEQ_METRICS (K3) or
+    one of fuzzy.SCORER (K3b).
     A functools.partial is "wlev" (weighted Levenshtein, its weights from _scorer_weights) or, with weights None or (w, w, w),
     "norm_lev"."""
     if scorer is None:
@@ -94,6 +107,7 @@ def _resolve_scorer(scorer, default, allow_jaro=False) -> str:
         raise NotImplementedError(f"scorer {scorer!r} is ambiguous: use 'osa' (optimal string alignment, restricted "
                                   "Damerau-Levenshtein) or 'dl' (unrestricted Damerau-Levenshtein)")
     raise NotImplementedError(f"scorer {scorer!r} has no GPU implementation (supported: 'ratio', 'levenshtein', 'osa', 'dl', "
+                              "'indel', 'lcsseq', 'hamming', 'prefix', 'postfix', "
                               f"{sorted(_FUZZ.values())}" + (", 'jaro_similarity', 'jaro_winkler_similarity'" if allow_jaro else "")
                               + "); polyfuzz_b200 has no CPU fallback")
 
@@ -282,7 +296,7 @@ class RapidFuzz(_KeepsTargets, BaseMatcher):
         same as a fresh call's); any call that stages keeps its to-side."""
         self_match = to_list is None
         targets = from_list if self_match else to_list
-        unit = self._metric in ("norm_lev", "norm_osa", "norm_dl", "wlev")     # scores already on 0..1
+        unit = self._metric in ("norm_lev", "norm_osa", "norm_dl", "wlev") + editdist.SEQ_METRICS     # scores already on 0..1
         scale = 1.0 if unit else 100.0
         cutoff = self.score_cutoff / 100.0 if unit else self.score_cutoff
         top_n = clip_top_n(self.top_n, to_list)
